@@ -160,12 +160,45 @@ tsgpu_status tsgpu_index_load_sort_column(tsgpu_index* idx, const int64_t* vals,
  * Index::index_field_in_memory src/index.cpp:1290-1400, Index::remove_field src/index.cpp:7295-7420). After a batch of writes the
  * binding hands over, in the form of tsgpu_index_load_field, the CURRENT full posting list of every token the batch touched (new
  * tokens included; an erased token = an empty list); they become lists *out_first_list .. *out_first_list + n_lists - 1 of `field`
- * and the caller points those tokens at the new ids. The lists they replace stay in HBM, unreferenced, until the field is loaded
- * again (the read-optimised layout has no holes to patch in place). seq_ids must stay below the n_docs the index was created with
- * (create it with headroom). Searches on other threads wait on the index lock for the duration of the call. */
+ * and the caller points those tokens at the new ids. The lists they replace stay in HBM, unreferenced, until the field is
+ * compacted (tsgpu_index_compact_field; the read-optimised layout has no holes to patch in place). seq_ids must stay below the
+ * index's capacity (tsgpu_index_create, raised by tsgpu_index_reserve_docs). Searches on other threads wait on the index lock for
+ * the duration of the call. */
 tsgpu_status tsgpu_index_append_lists(tsgpu_index* idx, uint32_t field, const tsgpu_field* f, uint32_t* out_first_list);
 /* sort_index values of upserted / removed documents: column[ids[i]] = vals[i] (INT64_MIN = no value). */
 tsgpu_status tsgpu_index_set_sort_values(tsgpu_index* idx, uint32_t sort_col, const uint32_t* ids, const int64_t* vals, size_t n);
+/* The garbage collection of the posting half of f-4: the field keeps only the lists live_lists[0 .. n_live-1] (the ones the
+ * binding's tokens still name — the reference's art_tree leaves, Index::search_index, whose posting_list_t replaced the old
+ * ones in place), and list live_lists[i] becomes list id i. Afterwards the field's arrays and flags are exactly what
+ * tsgpu_index_load_field builds from those lists in that order at the index's current capacity; the plain-field fast paths a
+ * replaced list had disabled come back. Nothing crosses PCIe but the list ids: the lists are gathered on the device, so the
+ * peak is the old field plus the new one. A list id >= n_lists or a duplicate is TSGPU_ERR_INVALID and leaves the field
+ * untouched. Needs the host's exclusive lock (as tsgpu_index_append_lists); list ids the caller held before are invalid after.
+ * tsgpu_get_stats afterwards: ms_kernels = device time of the gather, ms_total = the whole call on the stream. */
+tsgpu_status tsgpu_index_compact_field(tsgpu_index* idx, uint32_t field, const uint32_t* live_lists, uint32_t n_live);
+/* Raise the seq_id capacity to n_docs (Collection::get_next_seq_id, src/collection.cpp:101-104, only counts up: a live
+ * collection outgrows any capacity given at create time). Sort columns grow with INT64_MIN, persistent filters with zeros
+ * (their handles stay valid and exclude the new documents), dense posting bitmaps take the new stride, facet rows of the new
+ * documents are empty, the markDelete bitmap covers max(n_docs, graph nodes) and wildcard searches cover [0, n_docs). The
+ * all_result_ids kept by the last search are dropped. The same value is a no-op, a smaller one TSGPU_ERR_INVALID. The HNSW
+ * graph is not touched. Needs the host's exclusive lock. */
+tsgpu_status tsgpu_index_reserve_docs(tsgpu_index* idx, uint32_t n_docs);
+/* Shape of one mirrored field: what the host needs to decide when compaction pays (it knows how many lists are live). */
+#define TSGPU_FIELD_IS_ARRAY 1u          /* string[] field */
+#define TSGPU_FIELD_PLAIN_OK 2u          /* plain field, every posting's offsets well formed: the fast scoring path applies */
+#define TSGPU_FIELD_POS16 4u             /* ... and every position fits 16 bits */
+typedef struct {
+    uint32_t n_lists;                    /* list ids in use, live or replaced */
+    uint32_t flags;                      /* TSGPU_FIELD_* */
+    uint64_t n_postings;
+    uint64_t n_positions;
+    uint64_t n_blocks;                   /* packed id blocks */
+    uint64_t n_words;                    /* packed 32-bit words (without the padding word) */
+    uint32_t n_dense;                    /* lists that also have a bitmap */
+    uint32_t dense_words;                /* words per bitmap */
+    uint64_t device_bytes;               /* HBM held by the field's arrays */
+} tsgpu_field_info;
+tsgpu_status tsgpu_index_field_info(tsgpu_index* idx, uint32_t field, tsgpu_field_info* out);
 /* Mirror hnsw_index_t (vectors + graph). Pointers may be host or device memory. */
 tsgpu_status tsgpu_index_load_hnsw(tsgpu_index* idx, const tsgpu_hnsw* g);
 /* Build the vector index ON THE DEVICE: hnswlib's addPoint (the loop of Index::batch_memory_index, src/index.cpp:1003-1054,
@@ -408,6 +441,11 @@ typedef struct {
 tsgpu_status tsgpu_get_stats(tsgpu_index* idx, tsgpu_stats* out);
 /* Instrumentation: per graph walk of the last HNSW launch, out[2q] = expanded nodes, out[2q+1] = distance evaluations. */
 tsgpu_status tsgpu_debug_knn_work(tsgpu_index* idx, uint32_t* out, uint32_t cap_queries, uint32_t* out_n);
+/* Instrumentation: one of a field's ten device arrays over its logical length (bytes in *out_bytes; TSGPU_ERR_CAPACITY when
+ * cap_bytes is smaller). slot: 0 list_off, 1 list_blk_off, 2 blk_first, 3 blk_info, 4 packed (with its padding word), 5 pos_off,
+ * 6 positions, 7 list_dense, 8 dense_bits (with its 16 padding words), 9 dense_rank (with its padding entry); see
+ * csrc/postings_device.cuh. dst: host memory. */
+tsgpu_status tsgpu_debug_field_array(tsgpu_index* idx, uint32_t field, uint32_t slot, void* dst, size_t cap_bytes, size_t* out_bytes);
 
 #ifdef __cplusplus
 }

@@ -22,9 +22,20 @@ EXPORTS = [
     "tsgpu_index_load_sort_column", "tsgpu_index_append_lists", "tsgpu_index_set_sort_values", "tsgpu_index_load_hnsw", "tsgpu_index_build_hnsw", "tsgpu_index_append_hnsw", "tsgpu_index_mark_deleted", "tsgpu_index_hnsw_info", "tsgpu_index_export_hnsw", "tsgpu_filter_create", "tsgpu_filter_destroy", "tsgpu_filter_numeric", "tsgpu_filter_combine", "tsgpu_filter_ids", "tsgpu_scored_ids_search_batch",
     "tsgpu_intersect", "tsgpu_contains_atleast_one", "tsgpu_phrase_matches", "tsgpu_exact_matches", "tsgpu_prefix_matches", "tsgpu_ids_setop", "tsgpu_keyword_search_batch", "tsgpu_wildcard_search_batch", "tsgpu_knn_batch", "tsgpu_flat_distances", "tsgpu_flat_distances_batch",
     "tsgpu_vector_search_batch", "tsgpu_hybrid_search_batch", "tsgpu_get_stats", "tsgpu_debug_knn_work", "tsgpu_comm_unique_id", "tsgpu_comm_init", "tsgpu_comm_destroy", "tsgpu_comm_gather", "tsgpu_comm_last_ms", "tsgpu_hybrid_fuse_batch", "tsgpu_index_load_facet", "tsgpu_facet_counts", "tsgpu_facet_counts_last", "tsgpu_all_result_ids_last", "tsgpu_index_load_art", "tsgpu_art_walk_batch",
+    "tsgpu_index_compact_field", "tsgpu_index_reserve_docs", "tsgpu_index_field_info", "tsgpu_debug_field_array",
 ]
 
 
+class FieldInfoStruct(C.Structure):
+    """tsgpu_field_info"""
+    _fields_ = [("n_lists", C.c_uint32), ("flags", C.c_uint32), ("n_postings", C.c_uint64), ("n_positions", C.c_uint64), ("n_blocks", C.c_uint64),
+                ("n_words", C.c_uint64), ("n_dense", C.c_uint32), ("dense_words", C.c_uint32), ("device_bytes", C.c_uint64)]
+
+
+FIELD_IS_ARRAY, FIELD_PLAIN_OK, FIELD_POS16 = 1, 2, 4
+# tsgpu_debug_field_array slots: name and element type
+FIELD_ARRAYS = [("list_off", np.uint64), ("list_blk_off", np.uint32), ("blk_first", np.uint32), ("blk_info", np.uint64), ("packed", np.uint32),
+                ("pos_off", np.uint64), ("positions", np.uint32), ("list_dense", np.uint32), ("dense_bits", np.uint32), ("dense_rank", np.uint32)]
 FACET_DTYPE = np.dtype([("value_id", np.uint32), ("count", np.uint32), ("doc_id", np.uint32), ("array_pos", np.uint32)])
 QFLAG_KEEP_ALL_IDS = 0x80
 
@@ -58,6 +69,13 @@ def declare(L):
         L.tsgpu_index_load_sort_column.argtypes = [vp, C.c_void_p, u32p]
         L.tsgpu_index_append_lists.argtypes = [vp, C.c_uint32, C.POINTER(FieldStruct), u32p]
         L.tsgpu_index_set_sort_values.argtypes = [vp, C.c_uint32, C.c_void_p, C.c_void_p, C.c_size_t]
+        # the mirror maintenance calls: libtsgpu.so always has them; a library that re-exports an older C-ABI (the base test
+        # double, the host layer linked against it) may not, and then only calling them fails
+        for name, args in (("tsgpu_index_compact_field", [vp, C.c_uint32, C.c_void_p, C.c_uint32]), ("tsgpu_index_reserve_docs", [vp, C.c_uint32]),
+                           ("tsgpu_index_field_info", [vp, C.c_uint32, C.POINTER(FieldInfoStruct)]),
+                           ("tsgpu_debug_field_array", [vp, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)])):
+            if hasattr(L, name):
+                getattr(L, name).argtypes = args
         L.tsgpu_index_load_hnsw.argtypes = [vp, C.POINTER(HnswStruct)]
         L.tsgpu_index_build_hnsw.argtypes = [vp, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int]
         L.tsgpu_index_append_hnsw.argtypes = [vp, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]
@@ -169,6 +187,31 @@ class GpuIndex:
         ids = np.ascontiguousarray(ids, np.uint32)
         vals = np.ascontiguousarray(vals, np.int64)
         _ck(self.L.tsgpu_index_set_sort_values(self.h, col, ids.ctypes.data, vals.ctypes.data, len(ids)))
+
+    def compact_field(self, field: int, live_lists) -> None:
+        """tsgpu_index_compact_field: keep only `live_lists` (list live_lists[i] becomes list i) and free the rest."""
+        a = np.ascontiguousarray(live_lists, np.uint32)
+        _ck(self.L.tsgpu_index_compact_field(self.h, field, a.ctypes.data if len(a) else None, len(a)))
+
+    def reserve_docs(self, n_docs: int) -> None:
+        """tsgpu_index_reserve_docs: raise the seq_id capacity."""
+        _ck(self.L.tsgpu_index_reserve_docs(self.h, n_docs))
+        self.n_docs = n_docs
+
+    def field_info(self, field: int) -> dict:
+        s = FieldInfoStruct()
+        _ck(self.L.tsgpu_index_field_info(self.h, field, C.byref(s)))
+        return {n: getattr(s, n) for n, _ in FieldInfoStruct._fields_}
+
+    def field_array(self, field: int, slot: int) -> np.ndarray:
+        """tsgpu_debug_field_array: one of the field's ten device arrays (FIELD_ARRAYS) over its logical length."""
+        n = C.c_size_t(0)
+        rc = self.L.tsgpu_debug_field_array(self.h, field, slot, None, 0, C.byref(n))
+        if rc not in (0, 4):
+            _ck(rc)
+        out = np.zeros(max(n.value, 8), np.uint8)
+        _ck(self.L.tsgpu_debug_field_array(self.h, field, slot, out.ctypes.data, len(out), C.byref(n)))
+        return out[:n.value].view(FIELD_ARRAYS[slot][1]).copy()
 
     def load_field_raw(self, n_lists: int, is_array: bool, list_off, ids, pos_off, positions) -> int:
         """Pointers may be torch CUDA tensors (device-resident synthetic data)."""

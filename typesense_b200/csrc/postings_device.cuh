@@ -3,7 +3,8 @@
 // Replaces, for reading: posting_list_t::block_t + iterator_t (include/posting_list.h:56-127,
 // src/posting_list.cpp:1954-2061) and the FOR containers behind them (src/sorted_array.cpp, libfor).
 //
-// Layout per field (all arrays in HBM, built once by tsgpu_index_load_field):
+// Layout per field (all arrays in HBM, built by tsgpu_index_load_field, extended by tsgpu_index_append_lists, rebuilt by
+// tsgpu_index_compact_field as a gather of the live lists):
 //   list_off[L+1]      u64  posting index range of token list l            (-> pos_off, df = difference)
 //   list_blk_off[L+1]  u32  block index range of list l; blocks hold kBlock ids, only the last may be short
 //   blk_first[NB]      u32  first (= minimum) id of the block: the skip index (reference: id_block_map keyed by LAST id)
@@ -76,6 +77,24 @@ TS_HD uint32_t dense_rank_of(const DevField& f, uint32_t slot, uint32_t id) {
     if(wi >= 3) r += TS_POPC(b3 & m);
 #undef TS_POPC
     return r;
+}
+
+// The per-posting halves of kFieldPlainOk / kFieldPos16, shared by the loader (postings_pack.h) and the device-side
+// compaction (mirror_kernels.cuh) so the two cannot disagree. Raw offsets positions[a, b) of one posting are well formed
+// when they are strictly increasing, non-zero, optionally followed by one trailing 0 (src/index.cpp:1341-1348).
+TS_HD bool offsets_wellformed(const uint32_t* positions, uint64_t a, uint64_t b) {
+    if(b <= a) return false;
+    uint64_t e = b;
+    if(positions[b - 1] == 0) e = b - 1;
+    if(e <= a) return false;
+    uint32_t prev = 0;
+    for(uint64_t i = a; i < e; i++) { if(positions[i] == 0 || positions[i] <= prev) return false; prev = positions[i]; }
+    return true;
+}
+// no offset beyond 65535 (Match keeps offsets as uint16: beyond that they wrap)
+TS_HD bool offsets_fit_u16(const uint32_t* positions, uint64_t a, uint64_t b) {
+    for(uint64_t i = a; i < b; i++) if(positions[i] > 0xFFFFu) return false;
+    return true;
 }
 
 TS_HD uint32_t bits_required(uint32_t v) {

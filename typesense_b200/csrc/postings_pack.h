@@ -1,8 +1,9 @@
 // Host-side builder of the device posting layout (postings_device.cuh) from a flattened field (tsgpu_field).
-// Runs at mirror-load time only (the write path is out of scope; see DESIGN.md), never inside a search call.
+// Runs when a field is loaded or lists are appended (see DESIGN.md §7a), never inside a search call.
 #pragma once
 #include <stdint.h>
 #include <stddef.h>
+#include <algorithm>
 #include <vector>
 #include "postings_device.cuh"
 
@@ -96,22 +97,17 @@ inline void pack_field(uint32_t n_lists, const uint64_t* list_off, const uint32_
 // True when every posting of a plain string field has well-formed raw offsets: strictly increasing non-zero
 // positions, optionally followed by one trailing 0 (src/index.cpp:1341-1348). Enables score_field_plain().
 inline bool plain_wellformed(const uint64_t* pos_off, const uint32_t* positions, uint64_t n_post) {
-    for(uint64_t p = 0; p < n_post; p++) {
-        const uint64_t a = pos_off[p], b = pos_off[p + 1];
-        if(b <= a) return false;
-        uint64_t e = b;
-        if(positions[b - 1] == 0) e = b - 1;
-        if(e <= a) return false;
-        uint32_t prev = 0;
-        for(uint64_t i = a; i < e; i++) { if(positions[i] == 0 || positions[i] <= prev) return false; prev = positions[i]; }
-    }
+    for(uint64_t p = 0; p < n_post; p++) if(!tsdev::offsets_wellformed(positions, pos_off[p], pos_off[p + 1])) return false;
     return true;
 }
 
 // True when no position exceeds 65535 (Match keeps offsets as uint16: beyond that they wrap).
 inline bool positions_fit_u16(const uint32_t* positions, uint64_t n_positions) {
-    for(uint64_t i = 0; i < n_positions; i++) if(positions[i] > 0xFFFFu) return false;
-    return true;
+    return tsdev::offsets_fit_u16(positions, 0, n_positions);
 }
+
+// The dense-list threshold of a field: lists with at least this many postings get a bitmap. `div` is fixed per field at load
+// time (TSGPU_DENSE_DIV, default 64); n_docs is the index's capacity, which only grows.
+inline uint64_t dense_min_df(uint32_t n_docs, uint32_t div) { return std::max<uint64_t>(64, n_docs / (uint64_t) std::max<uint32_t>(1, div)); }
 
 }  // namespace tspack

@@ -22,7 +22,9 @@
 #include "knn_kernels.cuh"
 #include "hnsw_build.cuh"
 #include "facet_kernels.cuh"
+#include "mirror_kernels.cuh"
 #include "postings_pack.h"
+#include <cub/device/device_scan.cuh>
 
 // flat_tc.cu: the batched flat scan on the tensor cores (wgmma, tf32 x 3)
 extern "C" size_t tsgpu_flat_tc_image_bytes_(uint32_t ng, uint32_t dim, uint32_t* n_tile_out, uint32_t* n_qtiles_out);
@@ -104,9 +106,11 @@ struct FieldMirror {
     std::vector<uint32_t> h_list_dense;
     void* d_alloc[10] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     // element counts of the device arrays (tsgpu_index_append_lists grows them)
+    size_t d_bytes[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};   // bytes allocated per array (tsgpu_index_field_info)
     uint64_t n_post = 0, n_pos = 0, n_words = 0;      // postings, raw offsets, packed words (without the padding word)
     uint32_t n_blocks = 0, n_dense = 0;
     uint64_t dense_min_df = 0;
+    uint32_t dense_div = 64;                          // TSGPU_DENSE_DIV at load: the threshold is max(64, n_docs / dense_div)
 };
 
 struct Filter {
@@ -1121,9 +1125,12 @@ tsgpu_status tsgpu_index_load_field(tsgpu_index* idx, const tsgpu_field* f, uint
         cudaError_t e = cudaMalloc(&d, bytes ? bytes : 16);
         if(e != cudaSuccess) return e;
         fm.d_alloc[slot] = d;
+        fm.d_bytes[slot] = bytes ? bytes : 16;
         if(bytes) e = cudaMemcpy(d, src, bytes, from_user ? cudaMemcpyDefault : cudaMemcpyHostToDevice);
         return e;
     };
+    fm.dense_div = (uint32_t) std::max(1, getenv("TSGPU_DENSE_DIV") ? atoi(getenv("TSGPU_DENSE_DIV")) : 64);
+    fm.dense_min_df = tspack::dense_min_df(idx->n_docs, fm.dense_div);
     CU(up(0, fm.h_list_off.data(), ((size_t) L + 1) * 8, false));
     CU(up(1, pk.list_blk_off.data(), pk.list_blk_off.size() * 4, false));
     CU(up(2, pk.blk_first.data(), pk.blk_first.size() * 4, false));
@@ -1132,7 +1139,7 @@ tsgpu_status tsgpu_index_load_field(tsgpu_index* idx, const tsgpu_field* f, uint
     CU(up(5, f->pos_off, (n_post + 1) * 8, true));
     CU(up(6, f->positions, n_pos * 4, true));
     // dense lists: bitmap + rank directory (see postings_device.cuh)
-    tspack::pack_dense(L, fm.h_list_off.data(), h_ids.data(), idx->n_docs, std::max<uint64_t>(64, idx->n_docs / (uint64_t) std::max(1, getenv("TSGPU_DENSE_DIV") ? atoi(getenv("TSGPU_DENSE_DIV")) : 64)), pk);
+    tspack::pack_dense(L, fm.h_list_off.data(), h_ids.data(), idx->n_docs, fm.dense_min_df, pk);
     fm.h_list_dense = pk.list_dense;
     CU(up(7, pk.list_dense.data(), pk.list_dense.size() * 4, false));
     CU(up(8, pk.dense_bits.data(), pk.dense_bits.size() * 4, false));
@@ -1161,7 +1168,6 @@ tsgpu_status tsgpu_index_load_field(tsgpu_index* idx, const tsgpu_field* f, uint
     fm.dev.dense_rank = (const uint32_t*) fm.d_alloc[9];
     fm.dev.dense_words = pk.dense_words; fm.dev.dense_groups = pk.dense_groups;
     fm.n_post = n_post; fm.n_pos = n_pos; fm.n_words = pk.packed.size() - 1; fm.n_blocks = (uint32_t) pk.blk_first.size(); fm.n_dense = pk.n_dense;
-    fm.dense_min_df = std::max<uint64_t>(64, idx->n_docs / (uint64_t) std::max(1, getenv("TSGPU_DENSE_DIV") ? atoi(getenv("TSGPU_DENSE_DIV")) : 64));
     idx->ixdev.fields[idx->fields.size()] = fm.dev;
     *out_field = (uint32_t) idx->fields.size();
     idx->fields.push_back(std::move(fm));
@@ -1171,7 +1177,8 @@ tsgpu_status tsgpu_index_load_field(tsgpu_index* idx, const tsgpu_field* f, uint
 
 // SURVEY 8 f-4 (posting half). posting_t::upsert / erase (src/posting.cpp:247-333) change a token's list in place on the host; the
 // device layout is read-optimised (CSR + packed blocks), so a changed list is WRITTEN AGAIN at the end of the field's arrays and the
-// token is pointed at the new list id; the old list stays behind as garbage until the field is reloaded. Every array grows by
+// token is pointed at the new list id; the old list stays behind as garbage until the field is compacted (tsgpu_index_compact_field,
+// mirror_host.inc). Every array grows by
 // reallocation + device-to-device copy (O(field size) per call at HBM speed: batch the writes, as batch_memory_index does).
 tsgpu_status tsgpu_index_append_lists(tsgpu_index* idx, uint32_t field, const tsgpu_field* f, uint32_t* out_first_list) {
     tsgpu_status s = check_device(idx); if(s) return s;
@@ -1225,12 +1232,14 @@ tsgpu_status tsgpu_index_append_lists(tsgpu_index* idx, uint32_t field, const ts
     if(fm.n_words + nw_new >= (1ull << 40)) return fail(TSGPU_ERR_CAPACITY, "packed postings exceed the 40-bit word offset");
     // grow: [old | new] into fresh allocations, swap on success
     void* fresh[10] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    size_t fresh_bytes[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
     struct Guard { void** v; bool keep = false; ~Guard() { if(!keep) for(int i = 0; i < 10; i++) if(v[i]) cudaFree(v[i]); } } guard{fresh};
     auto grow = [&](int slot, size_t old_bytes, const void* add, size_t add_bytes, size_t tail_zero_bytes) -> cudaError_t {
         void* d = nullptr;
         cudaError_t e = cudaMalloc(&d, old_bytes + add_bytes + tail_zero_bytes + 16);
         if(e != cudaSuccess) return e;
         fresh[slot] = d;
+        fresh_bytes[slot] = old_bytes + add_bytes + tail_zero_bytes + 16;
         if(old_bytes) { e = cudaMemcpy(d, fm.d_alloc[slot], old_bytes, cudaMemcpyDeviceToDevice); if(e != cudaSuccess) return e; }
         if(add_bytes) { e = cudaMemcpy((char*) d + old_bytes, add, add_bytes, cudaMemcpyHostToDevice); if(e != cudaSuccess) return e; }
         if(tail_zero_bytes) e = cudaMemset((char*) d + old_bytes + add_bytes, 0, tail_zero_bytes);
@@ -1248,7 +1257,7 @@ tsgpu_status tsgpu_index_append_lists(tsgpu_index* idx, uint32_t field, const ts
     CU(grow(8, (size_t) fm.n_dense * dw * 4, pk.dense_bits.data(), (size_t) pk.n_dense * dw * 4, 64));
     CU(grow(9, (size_t) fm.n_dense * dg * 4, pk.dense_rank.data(), (size_t) pk.n_dense * dg * 4, 4));
     CU(cudaDeviceSynchronize());              // no search of this index is in flight (idx->mu), other indexes' streams finish first
-    for(int i = 0; i < 10; i++) { cudaFree(fm.d_alloc[i]); fm.d_alloc[i] = fresh[i]; }
+    for(int i = 0; i < 10; i++) { cudaFree(fm.d_alloc[i]); fm.d_alloc[i] = fresh[i]; fm.d_bytes[i] = fresh_bytes[i]; }
     guard.keep = true;
     fm.h_list_off.insert(fm.h_list_off.end(), lo.begin() + 1, lo.end());
     fm.h_list_blk_off.insert(fm.h_list_blk_off.end(), pk.list_blk_off.begin() + 1, pk.list_blk_off.end());
@@ -1381,6 +1390,7 @@ tsgpu_status tsgpu_index_load_hnsw(tsgpu_index* idx, const tsgpu_hnsw* g) {
 #include "hnsw_build_host.inc"
 #include "facet_host.inc"
 #include "comm_host.inc"
+#include "mirror_host.inc"
 
 tsgpu_status tsgpu_filter_create(tsgpu_index* idx, const uint32_t* ids, size_t n, int32_t* out_handle) {
     tsgpu_status s = check_device(idx); if(s) return s;

@@ -491,6 +491,50 @@ public:
         arts_ready.assign(arts_ready.size(), 0);                 // leaf max_score comes from the default sorting field
         return Option<bool>(true);
     }
+    // Frees the lists update_lists left behind: the field keeps the lists its tokens name, in ascending old id (so a field that was
+    // never patched keeps its ids), tokens are pointed at the new ids and the vocabulary drops the replaced lists. When to call it
+    // is the binding's decision (tsgpu_index_field_info says how many lists there are; token_ids how many are live). Like
+    // update_lists it needs the host's exclusive lock, and no multi_search_batched may be in flight: its passes hold list ids.
+    Option<bool> compact_field(const std::string& name) {
+        auto fit = field_ids.find(name);
+        if(fit == field_ids.end()) return Option<bool>(404, "no such field: " + name);
+        const uint32_t fid = fit->second;
+        std::vector<uint32_t> live;
+        live.reserve(token_ids[fid].size());
+        for(auto& p: token_ids[fid]) live.push_back(p.second);
+        std::sort(live.begin(), live.end());
+        if(tsgpu_index_compact_field(h, fid, live.empty() ? nullptr : live.data(), (uint32_t) live.size()) != TSGPU_OK)
+            return Option<bool>(500, tsgpu_last_error());
+        std::unordered_map<uint32_t, uint32_t> new_id;
+        new_id.reserve(live.size());
+        for(uint32_t i = 0; i < live.size(); i++) new_id[live[i]] = i;
+        for(auto& p: token_ids[fid]) p.second = new_id[p.second];
+        vocab_t& v = vocabs[fid];
+        vocab_t nv;
+        nv.tokens.reserve(live.size());
+        nv.list_off.assign(1, 0);
+        for(uint32_t l: live) {
+            nv.tokens.push_back(v.tokens[l]);
+            nv.ids.insert(nv.ids.end(), v.ids.begin() + (ptrdiff_t) v.list_off[l], v.ids.begin() + (ptrdiff_t) v.list_off[l + 1]);
+            nv.list_off.push_back(nv.ids.size());
+        }
+        v = std::move(nv);
+        arts_ready.assign(arts_ready.size(), 0);
+        { std::lock_guard<std::mutex> lk(cache_mu); walk_cache.clear(); }
+        return Option<bool>(true);
+    }
+    // Raises the seq_id capacity (Collection::get_next_seq_id only counts up): the binding calls it before it writes a document
+    // whose seq_id reaches the capacity. Sort columns gain documents without a value, filters gain documents outside them. Same
+    // lock rules as compact_field.
+    Option<bool> reserve_docs(uint32_t new_n_docs) {
+        if(tsgpu_index_reserve_docs(h, new_n_docs) != TSGPU_OK) return Option<bool>(400, tsgpu_last_error());
+        if(new_n_docs == n_docs) return Option<bool>(true);
+        for(auto& p: sort_values) p.second.resize(new_n_docs, INT64_MIN);
+        { std::lock_guard<std::mutex> lk(cache_mu); for(auto& p: host_filters) p.second.resize(((size_t) new_n_docs + 63) / 64, 0); }
+        n_docs = new_n_docs;
+        return Option<bool>(true);
+    }
+    uint32_t capacity() const { return n_docs; }
 
     // A filter_by result kept on the device (tsgpu_filter_create) with its host-side bit set: searches name it by handle, the
     // device applies it, and the host uses the bits where the reference consults the filter while it picks candidate tokens

@@ -9,6 +9,11 @@
 
 #include "tsgpu_host.hpp"
 
+// This wrapper is also linked against the oracle-backed test double of the C-ABI (the CPU arm), which has no mirror maintenance
+// calls: weak references let that build load, and its entry points report the missing call instead.
+#pragma weak tsgpu_index_compact_field
+#pragma weak tsgpu_index_reserve_docs
+
 namespace {
 thread_local std::string g_host_err;
 struct HostCtx { tsgpu::Index* ix; };
@@ -42,6 +47,20 @@ int tshost_add_sort_column(void* h, const char* name, const int64_t* dense_value
     auto op = IX(h).add_sort_field_dense(name, dense_values);
     if(!op.ok()) { g_host_err = op.error(); return -1; }
     return (int) op.get();
+}
+// f-4 maintenance: the lists a field's tokens no longer name are freed (Index::compact_field); the seq_id capacity grows
+// (Index::reserve_docs). 0 on success.
+int tshost_compact_field(void* h, const char* name) {
+    if(!tsgpu_index_compact_field) { g_host_err = "the linked tsgpu library has no tsgpu_index_compact_field"; return -1; }
+    auto op = IX(h).compact_field(name);
+    if(!op.ok()) { g_host_err = op.error(); return -1; }
+    return 0;
+}
+int tshost_reserve_docs(void* h, uint32_t n_docs) {
+    if(!tsgpu_index_reserve_docs) { g_host_err = "the linked tsgpu library has no tsgpu_index_reserve_docs"; return -1; }
+    auto op = IX(h).reserve_docs(n_docs);
+    if(!op.ok()) { g_host_err = op.error(); return -1; }
+    return 0;
 }
 int32_t tshost_add_filter(void* h, const uint32_t* ids, size_t n) {
     auto op = IX(h).add_filter(std::vector<uint32_t>(ids, ids + n));

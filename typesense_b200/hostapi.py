@@ -70,6 +70,8 @@ class HostIndex:
         L.tshost_tsgpu_handle.argtypes = [C.c_void_p]
         L.tshost_add_field_flat.argtypes = [C.c_void_p, C.c_char_p, C.c_uint32, C.c_char_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
         L.tshost_add_sort_column.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p]
+        L.tshost_compact_field.argtypes = [C.c_void_p, C.c_char_p]
+        L.tshost_reserve_docs.argtypes = [C.c_void_p, C.c_uint32]
         L.tshost_add_filter.restype = C.c_int32
         L.tshost_add_filter.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
         L.tshost_multi_search.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p, C.c_uint32, C.c_char_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32,
@@ -108,6 +110,17 @@ class HostIndex:
         if rc < 0:
             raise self._err()
         return rc
+
+    def compact_field(self, name: str) -> None:
+        """Index::compact_field: free the posting lists the field's tokens no longer name (needs the host's exclusive lock)."""
+        if self.L.tshost_compact_field(self.h, name.encode()) != 0:
+            raise self._err()
+
+    def reserve_docs(self, n_docs: int) -> None:
+        """Index::reserve_docs: raise the seq_id capacity."""
+        if self.L.tshost_reserve_docs(self.h, n_docs) != 0:
+            raise self._err()
+        self.n_docs = n_docs
 
     def add_filter(self, ids: np.ndarray) -> int:
         a = np.ascontiguousarray(ids, np.uint32)
