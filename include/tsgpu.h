@@ -36,7 +36,8 @@ enum {
 #define TSGPU_NO_LIST 0xFFFFFFFFu
 #define TSGPU_MAX_FIELDS 8      /* searched fields per query (reference: FIELD_LIMIT_NUM 100; see DESIGN.md) */
 #define TSGPU_MAX_TOKENS 16     /* token rows per combination (Match considers at most 10, include/match_score.h:11) */
-#define TSGPU_MAX_TOPK 1024     /* Topster capacity per query handled on device (DEFAULT_TOPSTER_SIZE 250) */
+#define TSGPU_MAX_TOPK 1024     /* Topster capacity per query of the shared-memory selection (DEFAULT_TOPSTER_SIZE 250); larger with
+                                   TSGPU_QFLAG_DEEP_TOPSTER (keyword, wildcard and scored-ids searches) */
 
 typedef struct tsgpu_index tsgpu_index;
 
@@ -87,12 +88,13 @@ typedef struct {
     const int32_t*  q_filter;          /* [nq]: -1 none; >=0 inline filter slot; <=-2 persistent handle -(v+2) */
     const uint32_t* q_excl_off;        /* [nq+1] -> excl_ids */
     const uint32_t* excl_ids;          /* sorted excluded_result_ids per query */
-    const uint32_t* q_topk;            /* [nq] Topster capacity (src/index.cpp:3506-3512), <= TSGPU_MAX_TOPK */
+    const uint32_t* q_topk;            /* [nq] Topster capacity (src/index.cpp:3506-3512), <= TSGPU_MAX_TOPK, or any value >= 1 with
+                                        * TSGPU_QFLAG_DEEP_TOPSTER; otherwise TSGPU_ERR_CAPACITY */
     const uint8_t*  q_sort_type;       /* [nq*3] TSGPU_SORT_* */
     const int32_t*  q_sort_col;        /* [nq*3] sort column for TSGPU_SORT_NUMERIC */
     const int8_t*   q_sort_order;      /* [nq*3] +1 desc, -1 asc (src/index.cpp:6853-6856) */
     const uint8_t*  q_sort_missing_first; /* [nq*3] or NULL */
-    const uint8_t*  q_flags;           /* [nq] TSGPU_FLAG_* */
+    const uint8_t*  q_flags;           /* [nq] TSGPU_FLAG_* | TSGPU_QFLAG_* */
     const uint8_t*  q_match_type;      /* [nq] */
     const uint8_t*  q_num_query_tokens;/* [nq] query_tokens.size() */
     const uint8_t*  q_field_weight;    /* [nq*F] search_field_t::weight */
@@ -387,6 +389,17 @@ tsgpu_status tsgpu_comm_last_ms(tsgpu_index* idx, float* out_ms);     /* device 
 /* tsgpu_kw_batch::q_flags bit: keep the query's all_result_ids (the id_buff / vec_search_ids union of src/index.cpp:5081-5090,
  * 4215-4219) on the device after a keyword / hybrid search, as one bit per doc — the `out_all_ids` of SURVEY 8(b). */
 #define TSGPU_QFLAG_KEEP_ALL_IDS 0x80u
+/* tsgpu_kw_batch::q_flags bit: the query may have q_topk > TSGPU_MAX_TOPK (deep pagination: page 40 at 250 per page needs a
+ * Topster of 10,000). Such a query's every match goes to a device buffer, which is then de-duplicated per seq_id and sorted;
+ * the memory this takes grows with the query's match count (at most the sum over its combinations of the driver list's
+ * postings; a wildcard or scored-ids query: its id count), not with q_topk. When that buffer cannot be allocated the call
+ * returns TSGPU_ERR_CAPACITY (the message gives the bytes) and the index stays usable. A buffer above 256 MiB is freed when the
+ * call returns; a smaller one stays with the index for the next call. With q_topk <= TSGPU_MAX_TOPK the
+ * flag changes nothing. Outputs keep their meaning: kv_stride truncates a query's records, out_found and query_index are
+ * as without the flag. Honoured by tsgpu_keyword_search_batch, tsgpu_wildcard_search_batch and
+ * tsgpu_scored_ids_search_batch; the vector and hybrid calls (tsgpu_vector_search_batch, tsgpu_hybrid_search_batch,
+ * tsgpu_hybrid_fuse_batch) reject it with TSGPU_ERR_INVALID, since their fusion keeps the Topster in shared memory. */
+#define TSGPU_QFLAG_DEEP_TOPSTER 0x20u
 /* Mirror of one facet field: facet_index_t's seq_id -> facet ids (src/facet_index.cpp:27-90; ids are the dense counter the
  * reference assigns per distinct value; a binding densifies numeric facets the same way). Host or device pointers. */
 typedef struct {
@@ -437,6 +450,12 @@ typedef struct {
     uint64_t calls_total;        /* C-ABI search calls since index creation */
     uint64_t knn_table_probes;   /* neighbour tests of the graph walks that missed the shared-memory visited cache (went to the HBM table) */
     uint64_t flat_tc_queries;    /* flat-path queries answered by the tensor-core scan (groups sharing a candidate set) in the last call */
+    uint64_t deep_entries;       /* entries the deep queries (TSGPU_QFLAG_DEEP_TOPSTER) of the last call emitted */
+    uint64_t deep_bytes;         /* device bytes the deep buffer of the last call needed */
+    float    ms_deep_emit;       /* unit kernels of the deep queries (also inside ms_kw_search) */
+    float    ms_deep_dedup;      /* de-duplication of the deep queries' entries per seq_id */
+    float    ms_deep_select;     /* sort of the distinct entries and the record write */
+    float    pad_deep;
 } tsgpu_stats;
 tsgpu_status tsgpu_get_stats(tsgpu_index* idx, tsgpu_stats* out);
 /* Instrumentation: per graph walk of the last HNSW launch, out[2q] = expanded nodes, out[2q+1] = distance evaluations. */

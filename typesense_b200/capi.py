@@ -38,6 +38,8 @@ FIELD_ARRAYS = [("list_off", np.uint64), ("list_blk_off", np.uint32), ("blk_firs
                 ("pos_off", np.uint64), ("positions", np.uint32), ("list_dense", np.uint32), ("dense_bits", np.uint32), ("dense_rank", np.uint32)]
 FACET_DTYPE = np.dtype([("value_id", np.uint32), ("count", np.uint32), ("doc_id", np.uint32), ("array_pos", np.uint32)])
 QFLAG_KEEP_ALL_IDS = 0x80
+QFLAG_DEEP_TOPSTER = 0x20       # q_topk may exceed MAX_TOPK (tsgpu_keyword / wildcard / scored_ids_search_batch)
+MAX_TOPK = 1024
 
 
 class TsgpuError(RuntimeError):

@@ -203,7 +203,10 @@ constexpr int kQCap = 2 * kThreads;        // pending-match queue slots per CTA
 // run-time indexed local arrays of score_field_plain(). <false> is the general scorer.
 // ONEFIELD (only instantiated next to REGSCORE): the batch searches a single field, so F is the constant 1 and the
 // per-row / per-field index arithmetic of narrowing, probing and scoring folds away.
-template <bool REGSCORE, bool ONEFIELD = false>
+// DEEP (deep_topster.cuh; kw_deep.cu launches it only over the units of deep queries, with KP = 0): no top-K buffer. Every scored match
+// goes to the query's slice of the deep buffer, which P.pool_* then address (64-bit index); P.q_thr[q] is the query's
+// cursor into it, starting at the slice's first entry. Match counts, found bitmaps and work counters are kept as here.
+template <bool REGSCORE, bool ONEFIELD = false, bool DEEP = false>
 __global__ void __launch_bounds__(kThreads, TSGPU_KW_MIN_CTAS)
 kw_search_kernel(const __grid_constant__ IndexDev ix, const __grid_constant__ KwParams P) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -284,7 +287,7 @@ kw_search_kernel(const __grid_constant__ IndexDev ix, const __grid_constant__ Kw
     // Scores queue entries [base, base+cnt) (cnt <= 128) with all threads busy, appends the survivors to the top-K
     // buffer and compacts that buffer when the next batch might not fit.
     auto score_batch = [&](uint32_t base, uint32_t cnt) {
-        const long long gthr = *reinterpret_cast<volatile long long*>(gthr_p);
+        const long long gthr = DEEP ? 0 : *reinterpret_cast<volatile long long*>(gthr_p);
         bool keep = false;
         int64_t sc[3] = {0, 0, 0};
         uint32_t mid = 0;
@@ -353,11 +356,24 @@ kw_search_kernel(const __grid_constant__ IndexDev ix, const __grid_constant__ Kw
             const int msi = compute_sort_scores(SS, mid, (int64_t) aggs, 0.0f, sc);
             if(msi >= 0) sc[msi] = (int64_t) aggs;            // src/index.cpp:5541-5544 (undoes the ASC negation)
             if(qd.found_bitmap) atomicOr(qd.found_bitmap + (mid >> 5), 1u << (mid & 31));
-            keep = sc[0] >= gthr;          // K distinct docs of this query already have scores[0] >= gthr
-            if(keep && s_have_thr) keep = kv_greater(sc[0], sc[1], sc[2], mid, thr[0], thr[1], thr[2], thr_key);
+            if constexpr (DEEP) keep = true;
+            else {
+                keep = sc[0] >= gthr;          // K distinct docs of this query already have scores[0] >= gthr
+                if(keep && s_have_thr) keep = kv_greater(sc[0], sc[1], sc[2], mid, thr[0], thr[1], thr[2], thr_key);
+            }
         }
         uint32_t a_total;
         const uint32_t arank = cta_rank(keep, s_warp, &a_total);
+        if constexpr (DEEP) {
+            // one atomic per CTA per batch reserves the batch's entries; thr[0] (unused here) carries the base
+            if(tid == 0 && a_total) thr[0] = (int64_t) atomicAdd(reinterpret_cast<unsigned long long*>(gthr_p), (unsigned long long) a_total);
+            __syncthreads();
+            if(keep) {
+                const size_t o = (size_t) thr[0] + arank;
+                P.pool_s0[o] = sc[0]; P.pool_s1[o] = sc[1]; P.pool_s2[o] = sc[2]; P.pool_key[o] = mid; P.pool_cmb[o] = cmb_local;
+            }
+            return;
+        }
         const uint32_t n0 = s_n;
         if(keep) {
             const uint32_t slot = n0 + arank;
@@ -564,7 +580,14 @@ kw_search_kernel(const __grid_constant__ IndexDev ix, const __grid_constant__ Kw
     }
 
     // ---- unit epilogue: best <= K entries to the pool
-    {
+    if constexpr (DEEP) {
+        if(tid == 0) {
+            if(s_matches) atomicAdd(P.combo_matches + ud.combo, s_matches);
+            atomicAdd(P.stats + 0, (unsigned long long) s_driver_ids);
+            atomicAdd(P.stats + 1, (unsigned long long) s_probe_blocks * kBlock);
+            atomicAdd(P.stats + 2, (unsigned long long) s_matches);
+        }
+    } else {
         const uint32_t n = s_n;
         uint32_t nn = n;
         if(n > 1) {                               // always sorted best-first: the merges read only the heads of their inputs
@@ -841,6 +864,9 @@ struct WcParams {
     uint32_t KP;
 };
 
+// DEEP: as kw_search_kernel<.., DEEP>: every matched id goes to the query's slice of the deep buffer (P.pool_*, cursor
+// P.q_thr[q]); launched with KP = 0 over the units of deep queries only.
+template <bool DEEP = false>
 __global__ void __launch_bounds__(kThreads)
 wc_unit_kernel(const __grid_constant__ WcParams P) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -878,13 +904,24 @@ wc_unit_kernel(const __grid_constant__ WcParams P) {
         if(keep) {
             const int64_t ms = (P.q_scores && P.q_scores[q]) ? __ldg(P.q_scores[q] + i) : 100;      // src/index.cpp:6727-6729; phrase-only: :6045
             compute_sort_scores(SS, id, ms, 0.0f, sc);
-            const long long gthr = *reinterpret_cast<volatile long long*>(gthr_p);
-            keep = sc[0] >= gthr;
-            if(keep && s_have_thr) keep = kv_greater(sc[0], sc[1], sc[2], id, thr[0], thr[1], thr[2], thr_key);
+            if constexpr (!DEEP) {
+                const long long gthr = *reinterpret_cast<volatile long long*>(gthr_p);
+                keep = sc[0] >= gthr;
+                if(keep && s_have_thr) keep = kv_greater(sc[0], sc[1], sc[2], id, thr[0], thr[1], thr[2], thr_key);
+            }
         }
         uint32_t m_total, a_total;
         cta_rank(matched, s_warp, &m_total);
         const uint32_t arank = cta_rank(keep, s_warp, &a_total);
+        if constexpr (DEEP) {
+            if(tid == 0) { s_matches += m_total; if(a_total) thr[0] = (int64_t) atomicAdd(reinterpret_cast<unsigned long long*>(gthr_p), (unsigned long long) a_total); }
+            __syncthreads();
+            if(keep) {
+                const size_t o = (size_t) thr[0] + arank;
+                P.pool_s0[o] = sc[0]; P.pool_s1[o] = sc[1]; P.pool_s2[o] = sc[2]; P.pool_key[o] = id; P.pool_cmb[o] = 0;
+            }
+            continue;
+        }
         const uint32_t n0 = s_n;
         if(keep) { const uint32_t slot = n0 + arank; tb.s0[slot] = sc[0]; tb.s1[slot] = sc[1]; tb.s2[slot] = sc[2]; tb.key[slot] = id; }
         __syncthreads();
@@ -907,6 +944,10 @@ wc_unit_kernel(const __grid_constant__ WcParams P) {
         }
     }
     __syncthreads();
+    if constexpr (DEEP) {
+        if(tid == 0 && s_matches) atomicAdd(P.combo_matches + q, s_matches);
+        return;
+    }
     const uint32_t n = s_n;
     uint32_t nn = n;
     if(n > 1) {                                   // always sorted best-first (see merge_units)

@@ -23,8 +23,11 @@
 #include "hnsw_build.cuh"
 #include "facet_kernels.cuh"
 #include "mirror_kernels.cuh"
+#include "deep_topster.cuh"
 #include "postings_pack.h"
+#include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
+#include <cub/device/device_select.cuh>
 
 // flat_tc.cu: the batched flat scan on the tensor cores (wgmma, tf32 x 3)
 extern "C" size_t tsgpu_flat_tc_image_bytes_(uint32_t ng, uint32_t dim, uint32_t* n_tile_out, uint32_t* n_qtiles_out);
@@ -39,6 +42,7 @@ using namespace tsk;
 extern "C" void tsgpu_art_release_(const tsgpu_index* idx);
 // kw_regscore.cu: kw_search_kernel<true> lives in its own translation unit (see there)
 extern "C" cudaError_t tsgpu_launch_kw_search_regscore(const void* index_dev, const void* kw_params, unsigned n_units, size_t smem, cudaStream_t st);
+extern "C" cudaError_t tsgpu_launch_kw_search_deep(const void* index_dev, const void* kw_params, unsigned n_units, size_t smem, cudaStream_t st);
 
 namespace {
 
@@ -151,11 +155,12 @@ struct tsgpu_index {
     void* comm = nullptr; int comm_rank = 0, comm_world = 1; float last_comm_ms = 0;       // ncclComm_t of tsgpu_comm_init
     int n_sms = 132;
     // scratch
-    DevBuf d_stage, d_pool, d_small, d_bitmaps, d_found_bm, d_out, d_knn_vis, d_knn_retry_vis, d_knn_retry_cand, d_knn_cand, d_knn_out, d_isect, d_kw_out;
+    DevBuf d_stage, d_pool, d_small, d_bitmaps, d_found_bm, d_out, d_knn_vis, d_knn_retry_vis, d_knn_retry_cand, d_knn_cand, d_knn_out, d_isect, d_kw_out, d_deep;
     PinBuf h_stage;
     size_t knn_slots = 0;
     bool found_dirty = false;            // d_found_bm is all-zero between calls unless a call died before its popcount pass
     cudaEvent_t ev[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    cudaEvent_t deep_ev[4] = {nullptr, nullptr, nullptr, nullptr};     // emit / de-duplicate / select of deep queries (created on first use)
     tsgpu_stats stats{};
 };
 
@@ -191,6 +196,13 @@ struct KwPlan {
     size_t n_inline_ids = 0;
     const int64_t* id_scores = nullptr;   // scored id sets (host or device, aligned with the batch's inline filter ids) or nullptr
     size_t pool_slots = 0;
+    // deep queries (TSGPU_QFLAG_DEEP_TOPSTER with topk > TSGPU_MAX_TOPK): their units, kept apart from everything that sizes the
+    // ordinary path, and their slices of the deep buffer, bounded by the entries they can emit
+    std::vector<uint32_t> deep_q;
+    std::vector<UDesc> deep_ud;
+    std::vector<unsigned long long> deep_off;  // [deep_q.size()+1] slice of deep query i in the deep buffer
+    unsigned long long deep_max = 0;           // largest slice
+    UDesc* d_deep_ud = nullptr; long long* d_deep_cur = nullptr;
     // device views (valid after upload)
     QDesc* d_qd = nullptr; CDesc* d_cd = nullptr; UDesc* d_ud = nullptr; uint32_t* d_multi_q = nullptr; uint32_t* d_multi_keep_q = nullptr;
     uint32_t* d_unit_cnt = nullptr; uint32_t* d_combo_matches = nullptr; unsigned long long* d_stats = nullptr;
@@ -303,11 +315,17 @@ tsgpu_status build_kw_plan(tsgpu_index* idx, const tsgpu_kw_batch* b, bool with_
     static const uint64_t unit_target = getenv("TSGPU_KW_UNIT_TARGET") ? (uint64_t) std::max(1, atoi(getenv("TSGPU_KW_UNIT_TARGET"))) : 8192;
     uint32_t tpu = (uint32_t) std::min<uint64_t>(256, std::max<uint64_t>(4, total_tiles / unit_target));
     std::vector<std::pair<uint32_t, uint32_t>> q_units0;
+    pl.deep_off.assign(1, 0);
     for(uint32_t q = 0; q < nq; q++) {
         QDesc& qd = pl.qd[q];
         const uint32_t K = b->q_topk[q];
-        if(K == 0 || K > TSGPU_MAX_TOPK) return fail(TSGPU_ERR_CAPACITY, "topk must be 1.." + std::to_string(TSGPU_MAX_TOPK));
-        qd.topk = K; kmax = std::max(kmax, K);
+        const bool deep_ok = (b->q_flags[q] & TSGPU_QFLAG_DEEP_TOPSTER) != 0;
+        if(K == 0 || (K > TSGPU_MAX_TOPK && !deep_ok))
+            return fail(TSGPU_ERR_CAPACITY, "topk must be 1.." + std::to_string(TSGPU_MAX_TOPK) + " (larger needs TSGPU_QFLAG_DEEP_TOPSTER)");
+        const bool deep = K > TSGPU_MAX_TOPK;
+        std::vector<UDesc>& uds = deep ? pl.deep_ud : pl.ud;
+        uint64_t deep_bound = 0;                  // entries a deep query can emit: one per matched (id, combination)
+        qd.topk = K; if(!deep) kmax = std::max(kmax, K);
         for(int i = 0; i < 3; i++) {
             qd.sort_type[i] = b->q_sort_type[q * 3 + i];
             qd.sort_order[i] = b->q_sort_order[q * 3 + i];
@@ -319,7 +337,7 @@ tsgpu_status build_kw_plan(tsgpu_index* idx, const tsgpu_kw_batch* b, bool with_
                 qd.sort_col[i] = idx->sort_cols[col];
             }
         }
-        qd.flags = b->q_flags[q] & 0x3F; qd.rerank = (b->q_flags[q] & TSGPU_FLAG_RERANK_HYBRID_MATCHES) ? 1 : 0; qd.match_type = b->q_match_type[q]; qd.num_query_tokens = b->q_num_query_tokens[q];
+        qd.flags = b->q_flags[q] & 0x1F; qd.rerank = (b->q_flags[q] & TSGPU_FLAG_RERANK_HYBRID_MATCHES) ? 1 : 0; qd.match_type = b->q_match_type[q]; qd.num_query_tokens = b->q_num_query_tokens[q];
         qd.keep_all = (b->q_flags[q] & TSGPU_QFLAG_KEEP_ALL_IDS) ? 1 : 0;
         for(uint32_t f = 0; f < (uint32_t) kMaxFieldSlots; f++) qd.field_weight[f] = f < F ? b->q_field_weight[(size_t) q * F + f] : 0;
         qd.n_excl = b->q_excl_off[q + 1] - b->q_excl_off[q];
@@ -332,12 +350,13 @@ tsgpu_status build_kw_plan(tsgpu_index* idx, const tsgpu_kw_batch* b, bool with_
             pl.cd[c].q = q;
             if(combo_tiles[c]) combos_with_tiles++;
             const uint32_t ctpu = pl.cd[c].mode == 1 ? 64u : tpu;      // a dense tile is 4096 docs of bitmap words
+            if(deep) deep_bound += std::min<uint64_t>((uint64_t) combo_tiles[c] * (pl.cd[c].mode == 1 ? 4096u : 128u), idx->n_docs);
             for(uint32_t t = 0; t < combo_tiles[c]; t += ctpu) {
                 UDesc u;
                 u.combo = c; u.tile_begin = t; u.tile_end = std::min(combo_tiles[c], t + ctpu);
-                u.out_off = (uint32_t) pl.pool_slots;
-                pl.pool_slots += K;
-                pl.ud.push_back(u);
+                u.out_off = deep ? 0u : (uint32_t) pl.pool_slots;
+                if(!deep) pl.pool_slots += K;
+                uds.push_back(u);
             }
         }
         if(wildcard) {
@@ -351,15 +370,21 @@ tsgpu_status build_kw_plan(tsgpu_index* idx, const tsgpu_kw_batch* b, bool with_
             pl.n_inline_ids = b->n_filters ? (size_t) b->filter_off[b->n_filters] : 0;
             qd.combo_begin = q; qd.combo_end = q + 1;
             const uint32_t tiles = (uint32_t) ((n_ids + kThreads - 1) / kThreads), wtpu = 64;
+            if(deep) deep_bound = n_ids;
             for(uint32_t t = 0; t < tiles; t += wtpu) {
                 UDesc u;
                 u.combo = q; u.tile_begin = t; u.tile_end = std::min(tiles, t + wtpu);
-                u.out_off = (uint32_t) pl.pool_slots;
-                pl.pool_slots += K;
-                pl.ud.push_back(u);
+                u.out_off = deep ? 0u : (uint32_t) pl.pool_slots;
+                if(!deep) pl.pool_slots += K;
+                uds.push_back(u);
             }
         }
         qd.unit_end = (uint32_t) pl.ud.size();
+        if(deep) {
+            pl.deep_q.push_back(q);
+            pl.deep_off.push_back(pl.deep_off.back() + deep_bound);
+            pl.deep_max = std::max<unsigned long long>(pl.deep_max, deep_bound);
+        }
         q_units0.push_back({qd.unit_begin, qd.unit_end});
         if(qd.keep_all && !wildcard) { pl.keep_q.push_back(q); if(combos_with_tiles > 1) pl.multi_keep_q.push_back(q); }
         else if(combos_with_tiles > 1) pl.multi_q.push_back(q);
@@ -447,6 +472,8 @@ tsgpu_status upload_kw_plan(tsgpu_index* idx, const tsgpu_kw_batch* b, KwPlan& p
     for(auto& lv: pl.levels) o_lv.push_back(sg.add(lv.data(), lv.size() * sizeof(MDesc)));
     const size_t o_cnt = sg.reserve(((size_t) pl.n_units_total + pl.nc + 8) * 4 + 64);
     const size_t o_thr = sg.reserve((size_t) nq * 8);
+    const size_t o_dud = sg.add(pl.deep_ud.data(), pl.deep_ud.size() * sizeof(UDesc));
+    const size_t o_dcur = sg.reserve(pl.deep_q.empty() ? 0 : (size_t) nq * 8);
     CU(idx->d_stage.reserve(sg.host.size()));
     unsigned char* dbase = idx->d_stage.as<unsigned char>();
     const uint32_t* d_excl = reinterpret_cast<const uint32_t*>(dbase + o_excl);
@@ -483,6 +510,11 @@ tsgpu_status upload_kw_plan(tsgpu_index* idx, const tsgpu_kw_batch* b, KwPlan& p
     memcpy(sg.host.data() + o_mk, pl.multi_keep_q.data(), pl.multi_keep_q.size() * 4);
     memset(sg.host.data() + o_cnt, 0, ((size_t) pl.n_units_total + pl.nc + 8) * 4 + 64);
     for(uint32_t q = 0; q < nq; q++) reinterpret_cast<long long*>(sg.host.data() + o_thr)[q] = INT64_MIN;
+    if(!pl.deep_q.empty()) {                  // deep cursors start at their slices
+        long long* cur = reinterpret_cast<long long*>(sg.host.data() + o_dcur);
+        for(uint32_t q = 0; q < nq; q++) cur[q] = 0;
+        for(size_t i = 0; i < pl.deep_q.size(); i++) cur[pl.deep_q[i]] = (long long) pl.deep_off[i];
+    }
     CU(idx->h_stage.reserve(sg.host.size()));
     memcpy(idx->h_stage.p, sg.host.data(), sg.host.size());
     CU(cudaMemcpyAsync(dbase, idx->h_stage.p, sg.host.size(), cudaMemcpyHostToDevice, st));
@@ -499,6 +531,8 @@ tsgpu_status upload_kw_plan(tsgpu_index* idx, const tsgpu_kw_batch* b, KwPlan& p
     pl.d_combo_matches = reinterpret_cast<uint32_t*>(cnt + 32);
     pl.d_unit_cnt = pl.d_combo_matches + pl.nc;
     pl.d_q_thr = reinterpret_cast<long long*>(dbase + o_thr);
+    pl.d_deep_ud = reinterpret_cast<UDesc*>(dbase + o_dud);
+    pl.d_deep_cur = reinterpret_cast<long long*>(dbase + o_dcur);
     // inline filter bitmaps
     for(size_t s = 0; s < n_inline; s++) {
         const size_t n = (size_t) (b->filter_off[s + 1] - b->filter_off[s]);
@@ -510,10 +544,103 @@ tsgpu_status upload_kw_plan(tsgpu_index* idx, const tsgpu_kw_batch* b, KwPlan& p
     return TSGPU_OK;
 }
 
-size_t kw_search_smem(const KwPlan& pl) { return (size_t) 2 * pl.KP * 28 + (size_t) pl.NL * kThreads * 4 + (size_t) kQCap * 4 + (size_t) pl.NL * kQCap * 4; }
+size_t kw_search_smem(uint32_t KP, uint32_t NL) { return (size_t) 2 * KP * 28 + (size_t) NL * kThreads * 4 + (size_t) kQCap * 4 + (size_t) NL * kQCap * 4; }
 size_t kw_final_smem(const KwPlan& pl) { return (size_t) 2 * pl.KP * 30 + 16; }
 
 struct KwDeviceOut { KVOut* kv; uint32_t* count; uint32_t* found; uint32_t* searched; uint32_t stride; };
+
+// The deep buffer: the deep queries' emitted slices (structure of arrays, 30 bytes an entry, 64-bit index), then two
+// DeepEntry arrays and the head flags for the largest slice, then CUB's scratch. Sized by the plan's upper bounds before
+// anything runs; when it cannot be allocated the call fails with TSGPU_ERR_CAPACITY and the index stays usable.
+constexpr size_t kDeepKeepBytes = size_t(256) << 20;
+
+struct DeepBuf {
+    int64_t *s0 = nullptr, *s1 = nullptr, *s2 = nullptr; uint32_t* key = nullptr; uint16_t* cmb = nullptr;
+    DeepEntry *a = nullptr, *b = nullptr; uint8_t* head = nullptr; unsigned long long* n_sel = nullptr;
+    void* temp = nullptr; size_t temp_bytes = 0;
+};
+
+tsgpu_status deep_reserve(tsgpu_index* idx, const KwPlan& pl, DeepBuf& db) {
+    const size_t T = pl.deep_off.back(), M = pl.deep_max;
+    size_t t1 = 0, t2 = 0, t3 = 0;
+    DeepEntry* const none = nullptr;
+    CU(cub::DeviceRadixSort::SortKeysDescending(nullptr, t1, none, none, M, DeepKvOrder{}));
+    CU(cub::DeviceRadixSort::SortKeysDescending(nullptr, t2, none, none, M, DeepKeyOrder{}));
+    CU(cub::DeviceSelect::Flagged(nullptr, t3, none, static_cast<const uint8_t*>(nullptr), none, static_cast<unsigned long long*>(nullptr), M));
+    db.temp_bytes = std::max(t1, std::max(t2, t3));
+    size_t off = 0;
+    auto take = [&](size_t bytes) { const size_t o = off; off = (off + bytes + 255) & ~size_t(255); return o; };
+    const size_t o0 = take(T * 8), o1 = take(T * 8), o2 = take(T * 8), ok = take(T * 4), oc = take(T * 2);
+    const size_t oa = take(M * sizeof(DeepEntry)), ob = take(M * sizeof(DeepEntry)), oh = take(M), on = take(8), ot = take(db.temp_bytes);
+    idx->stats.deep_bytes = off;
+    if(idx->d_deep.reserve(off) != cudaSuccess) {
+        cudaGetLastError();                   // an allocation failure is not sticky: clear it so the next call starts clean
+        return fail(TSGPU_ERR_CAPACITY, "deep Topster needs " + std::to_string(off) + " bytes of device memory; lower topk or split the batch");
+    }
+    unsigned char* p = idx->d_deep.as<unsigned char>();
+    db.s0 = reinterpret_cast<int64_t*>(p + o0); db.s1 = reinterpret_cast<int64_t*>(p + o1); db.s2 = reinterpret_cast<int64_t*>(p + o2);
+    db.key = reinterpret_cast<uint32_t*>(p + ok); db.cmb = reinterpret_cast<uint16_t*>(p + oc);
+    db.a = reinterpret_cast<DeepEntry*>(p + oa); db.b = reinterpret_cast<DeepEntry*>(p + ob);
+    db.head = p + oh; db.n_sel = reinterpret_cast<unsigned long long*>(p + on); db.temp = p + ot;
+    return TSGPU_OK;
+}
+
+// After the unit kernels: de-duplicate, select and write every deep query's Topster (deep_topster.cuh). The entry counts
+// come back to the host first, so the sorts are sized by what was emitted, not by the bound.
+tsgpu_status run_deep_select(tsgpu_index* idx, const KwPlan& pl, DeepBuf& db, const KwDeviceOut& out) {
+    cudaStream_t st = idx->stream;
+    std::vector<long long> cur(pl.nq);
+    std::vector<uint32_t> cm(pl.nc);
+    CU(cudaMemcpyAsync(cur.data(), pl.d_deep_cur, (size_t) pl.nq * 8, cudaMemcpyDeviceToHost, st));
+    if(pl.nc) CU(cudaMemcpyAsync(cm.data(), pl.d_combo_matches, (size_t) pl.nc * 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    const unsigned grid_cap = (unsigned) idx->n_sms * 8;
+    auto grid = [&](size_t n) { return (unsigned) std::max<size_t>(1, std::min<size_t>((n + 255) / 256, grid_cap)); };
+    float ms_dedup = 0, ms_select = 0;
+    for(size_t i = 0; i < pl.deep_q.size(); i++) {
+        const uint32_t q = pl.deep_q[i];
+        const QDesc& qd = pl.qd[q];
+        const size_t base = pl.deep_off[i];
+        size_t n = (size_t) cur[q] - base;
+        idx->stats.deep_entries += n;
+        if(n == 0) continue;                  // kw_final_kernel wrote count 0
+        uint32_t with_matches = 0;
+        for(uint32_t c = qd.combo_begin; c < qd.combo_end; c++) with_matches += cm[c] != 0;
+        const bool dedup = with_matches > 1;
+        CU(cudaEventRecord(idx->deep_ev[1], st));
+        deep_pack_kernel<<<grid(n), 256, 0, st>>>(db.s0 + base, db.s1 + base, db.s2 + base, db.key + base, db.cmb + base, n, dedup ? 1 : 0, db.a);
+        idx->stats.launches_total++;
+        CU(cudaGetLastError());
+        if(dedup) {
+            size_t tb = db.temp_bytes;
+            CU(cub::DeviceRadixSort::SortKeysDescending(db.temp, tb, db.a, db.b, n, DeepKeyOrder{}, st));
+            deep_heads_kernel<<<grid(n), 256, 0, st>>>(db.b, n, db.a, db.head);
+            idx->stats.launches_total++;
+            CU(cudaGetLastError());
+            tb = db.temp_bytes;
+            CU(cub::DeviceSelect::Flagged(db.temp, tb, db.a, static_cast<const uint8_t*>(db.head), db.b, db.n_sel, n, st));
+            unsigned long long n_sel = 0;
+            CU(cudaMemcpyAsync(&n_sel, db.n_sel, 8, cudaMemcpyDeviceToHost, st));
+            CU(cudaStreamSynchronize(st));
+            n = (size_t) n_sel;
+            std::swap(db.a, db.b);            // the distinct entries are in a
+        }
+        CU(cudaEventRecord(idx->deep_ev[2], st));
+        size_t tb = db.temp_bytes;
+        CU(cub::DeviceRadixSort::SortKeysDescending(db.temp, tb, db.a, db.b, n, DeepKvOrder{}, st));
+        const uint32_t n_out = (uint32_t) std::min<size_t>(n, std::min(qd.topk, out.stride));
+        deep_write_kernel<<<grid(n_out), 256, 0, st>>>(db.b, n_out, pl.d_qd, q, pl.d_combo_matches, out.kv, out.stride, out.count);
+        idx->stats.launches_total++;
+        CU(cudaGetLastError());
+        CU(cudaEventRecord(idx->deep_ev[3], st));
+        CU(cudaEventSynchronize(idx->deep_ev[3]));
+        float ms = 0;
+        cudaEventElapsedTime(&ms, idx->deep_ev[1], idx->deep_ev[2]); ms_dedup += ms;
+        cudaEventElapsedTime(&ms, idx->deep_ev[2], idx->deep_ev[3]); ms_select += ms;
+    }
+    idx->stats.ms_deep_dedup = ms_dedup; idx->stats.ms_deep_select = ms_select;
+    return TSGPU_OK;
+}
 
 // intersect/score/select + per-query merge; leaves KVOut/count/found/searched in idx->d_kw_out
 tsgpu_status run_keyword(tsgpu_index* idx, KwPlan& pl, uint32_t kv_stride, KwDeviceOut& out) {
@@ -532,8 +659,15 @@ tsgpu_status run_keyword(tsgpu_index* idx, KwPlan& pl, uint32_t kv_stride, KwDev
     int64_t* p2 = p1 + pl.pool_slots;
     uint32_t* pk = reinterpret_cast<uint32_t*>(p2 + pl.pool_slots);
     uint16_t* pc = reinterpret_cast<uint16_t*>(pk + pl.pool_slots);
+    const bool deep = !pl.deep_q.empty();
+    DeepBuf db;
+    if(deep) {
+        tsgpu_status s = deep_reserve(idx, pl, db); if(s) return s;
+        for(auto& e: idx->deep_ev) if(!e) CU(cudaEventCreate(&e));
+    }
+    const unsigned n_deep_units = (unsigned) pl.deep_ud.size();
     CU(cudaEventRecord(idx->ev[1], st));
-    if(pl.n_units && pl.wildcard) {
+    if((pl.n_units || n_deep_units) && pl.wildcard) {
         // per-query id arrays
         std::vector<const uint32_t*> qids(nq);
         for(uint32_t q = 0; q < nq; q++) qids[q] = pl.q_filter_ids[q];
@@ -560,11 +694,21 @@ tsgpu_status run_keyword(tsgpu_index* idx, KwPlan& pl, uint32_t kv_stride, KwDev
         P.pool_s0 = p0; P.pool_s1 = p1; P.pool_s2 = p2; P.pool_key = pk; P.pool_cmb = pc;
         P.unit_cnt = pl.d_unit_cnt; P.combo_matches = pl.d_combo_matches; P.q_thr = pl.d_q_thr; P.KP = pl.KP;
         const size_t smem = (size_t) 2 * pl.KP * 28;
-        CU(cudaFuncSetAttribute(wc_unit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) std::max<size_t>(smem, 48 * 1024)));
-        wc_unit_kernel<<<pl.n_units, kThreads, smem, st>>>(P);
-        idx->stats.launches_total++;
-        CU(cudaGetLastError());
-    } else if(pl.n_units) {
+        if(pl.n_units) {
+            CU(cudaFuncSetAttribute(wc_unit_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) std::max<size_t>(smem, 48 * 1024)));
+            wc_unit_kernel<false><<<pl.n_units, kThreads, smem, st>>>(P);
+            idx->stats.launches_total++;
+            CU(cudaGetLastError());
+        }
+        if(n_deep_units) {
+            P.ud = pl.d_deep_ud; P.q_thr = pl.d_deep_cur; P.KP = 0;
+            P.pool_s0 = db.s0; P.pool_s1 = db.s1; P.pool_s2 = db.s2; P.pool_key = db.key; P.pool_cmb = db.cmb;
+            CU(cudaEventRecord(idx->deep_ev[0], st));
+            wc_unit_kernel<true><<<n_deep_units, kThreads, 0, st>>>(P);
+            idx->stats.launches_total++;
+            CU(cudaGetLastError());
+        }
+    } else if(pl.n_units || n_deep_units) {
         KwParams P{};
         P.qd = pl.d_qd; P.cd = pl.d_cd; P.ud = pl.d_ud;
         P.pool_s0 = p0; P.pool_s1 = p1; P.pool_s2 = p2; P.pool_key = pk; P.pool_cmb = pc;
@@ -572,15 +716,24 @@ tsgpu_status run_keyword(tsgpu_index* idx, KwPlan& pl, uint32_t kv_stride, KwDev
         P.q_thr = pl.d_q_thr;
         P.F = pl.F; P.KP = pl.KP; P.NL = pl.NL;
         for(uint32_t f = 0; f < (uint32_t) kMaxFieldSlots; f++) P.field_ids[f] = pl.field_ids[f];
-        const size_t smem = kw_search_smem(pl);
-        static const bool reg_score = !(getenv("TSGPU_REG_SCORE") && atoi(getenv("TSGPU_REG_SCORE")) == 0);   // default; =0 selects the general scorer (kw_search_kernel<false>) for A/B
-        if(reg_score) CU(tsgpu_launch_kw_search_regscore(&idx->ixdev, &P, pl.n_units, smem, st));          // kw_regscore.cu
-        else {
-            CU(cudaFuncSetAttribute(kw_search_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) std::max<size_t>(smem, 48 * 1024)));
-            kw_search_kernel<false><<<pl.n_units, kThreads, smem, st>>>(idx->ixdev, P);
+        if(pl.n_units) {
+            const size_t smem = kw_search_smem(pl.KP, pl.NL);
+            static const bool reg_score = !(getenv("TSGPU_REG_SCORE") && atoi(getenv("TSGPU_REG_SCORE")) == 0);   // default; =0 selects the general scorer (kw_search_kernel<false>) for A/B
+            if(reg_score) CU(tsgpu_launch_kw_search_regscore(&idx->ixdev, &P, pl.n_units, smem, st));          // kw_regscore.cu
+            else {
+                CU(cudaFuncSetAttribute(kw_search_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) std::max<size_t>(smem, 48 * 1024)));
+                kw_search_kernel<false><<<pl.n_units, kThreads, smem, st>>>(idx->ixdev, P);
+            }
+            idx->stats.launches_total++;
+            CU(cudaGetLastError());
         }
-        idx->stats.launches_total++;
-        CU(cudaGetLastError());
+        if(n_deep_units) {                    // the register-resident scorer without the top-K buffer (kw_deep.cu)
+            P.ud = pl.d_deep_ud; P.q_thr = pl.d_deep_cur; P.KP = 0;
+            P.pool_s0 = db.s0; P.pool_s1 = db.s1; P.pool_s2 = db.s2; P.pool_key = db.key; P.pool_cmb = db.cmb;
+            CU(cudaEventRecord(idx->deep_ev[0], st));
+            CU(tsgpu_launch_kw_search_deep(&idx->ixdev, &P, n_deep_units, kw_search_smem(0, pl.NL), st));
+            idx->stats.launches_total++;
+        }
     }
     CU(cudaEventRecord(idx->ev[6], st));
     {
@@ -617,6 +770,15 @@ tsgpu_status run_keyword(tsgpu_index* idx, KwPlan& pl, uint32_t kv_stride, KwDev
             idx->stats.launches_total++;
             CU(cudaGetLastError());
         }
+    }
+    if(deep) {
+        // kw_final_kernel gave the deep queries (no ordinary units) their found / query counts and count 0; the selection
+        // below writes their records and count
+        tsgpu_status s = run_deep_select(idx, pl, db, out); if(s) return s;
+        if(n_deep_units) cudaEventElapsedTime(&idx->stats.ms_deep_emit, idx->deep_ev[0], idx->ev[6]);
+        // run_deep_select has waited for its last kernel: a large deep buffer goes back to the device at once rather than
+        // staying with the index (a q=* over 10 M documents needs 1.3 GB); small ones are kept for the next call
+        if(idx->d_deep.cap > kDeepKeepBytes) idx->d_deep.release();
     }
     CU(cudaEventRecord(idx->ev[2], st));
     return TSGPU_OK;
@@ -1084,10 +1246,11 @@ void tsgpu_index_destroy(tsgpu_index* idx) {
     idx->d_keep_bm.release(); idx->d_facet.release(); idx->d_comm.release();
     if(idx->comm) { tsgpu_comm_destroy(idx); }
     DevBuf* bufs[] = {&idx->d_stage, &idx->d_pool, &idx->d_small, &idx->d_bitmaps, &idx->d_found_bm, &idx->d_out, &idx->d_knn_vis,
-                      &idx->d_knn_retry_vis, &idx->d_knn_retry_cand, &idx->d_knn_cand, &idx->d_knn_out, &idx->d_isect, &idx->d_kw_out};
+                      &idx->d_knn_retry_vis, &idx->d_knn_retry_cand, &idx->d_knn_cand, &idx->d_knn_out, &idx->d_isect, &idx->d_kw_out, &idx->d_deep};
     for(auto* b: bufs) b->release();
     idx->h_stage.release();
     for(auto& e: idx->ev) if(e) cudaEventDestroy(e);
+    for(auto& e: idx->deep_ev) if(e) cudaEventDestroy(e);
     if(idx->evA) cudaEventDestroy(idx->evA);
     if(idx->evB) cudaEventDestroy(idx->evB);
     if(idx->stream2) cudaStreamDestroy(idx->stream2);
@@ -1900,6 +2063,8 @@ static tsgpu_status vec_or_hybrid(tsgpu_index* idx, const tsgpu_kw_batch* b, con
     tsgpu_status s = check_device(idx); if(s) return s;
     if(!b || !qvecs || !vp || !out_kv || !out_count || !out_found || kv_stride == 0) return fail(TSGPU_ERR_INVALID, "null argument");
     if(!idx->has_hnsw) return fail(TSGPU_ERR_INVALID, "no vector index loaded");
+    for(uint32_t q = 0; q < b->n_queries; q++)         // the fusion kernel holds its Topster in shared memory
+        if(b->q_flags[q] & TSGPU_QFLAG_DEEP_TOPSTER) return fail(TSGPU_ERR_INVALID, "TSGPU_QFLAG_DEEP_TOPSTER is not supported by vector and hybrid searches");
     std::lock_guard<std::mutex> lk(idx->mu);
     begin_call(idx);
     KwPlan pl;

@@ -708,7 +708,6 @@ public:
         q.has_filter = filter_by_provided;
         q.filter_ids = filter_ids;
         q.excl = excluded_result_ids;
-        q.topk = (uint32_t) std::min<size_t>(topster_size, TSGPU_MAX_TOPK);
         for(size_t i = 0; i < sort_fields.size() && i < 3; i++) {
             q.sort_type[i] = (uint8_t) sort_fields[i].type;
             q.sort_order[i] = sort_fields[i].desc ? 1 : -1;
@@ -718,6 +717,7 @@ public:
         q.flags = (uint8_t) ((prioritize_exact_match ? TSGPU_FLAG_PRIORITIZE_EXACT_MATCH : 0) |
                              (prioritize_token_position ? TSGPU_FLAG_PRIORITIZE_TOKEN_POSITION : 0) |
                              (prioritize_num_matching_fields ? TSGPU_FLAG_PRIORITIZE_NUM_MATCHING_FIELDS : 0));
+        size_topster(q, topster_size);
         q.match_type = (uint8_t) text_match_type;
         q.nqt = (uint8_t) n_query_tokens;
         q.field_weights = field_weights;
@@ -725,6 +725,24 @@ public:
         q.c_orig.assign(query_suggestions.size(), orig_num_tokens);
         q.c_flags.assign(query_suggestions.size(), (uint8_t) ((is_synonym_query ? TSGPU_CFLAG_SYNONYM : 0) | (demote_synonym_match ? TSGPU_CFLAG_DEMOTE_SYNONYM : 0)));
         return q;
+    }
+    // Topster capacity of a keyword, wildcard or phrase-only query. Above TSGPU_MAX_TOPK (deep pagination) the query takes the
+    // device's deep path, with the reference's own cap (src/index.cpp:3507-3510): no Topster holds more distinct keys than the
+    // collection has documents or the filter has ids, so the cap changes no result and bounds the device buffers.
+    uint32_t deep_topk(size_t topster_size, const std::vector<uint32_t>* filter_ids) const {
+        size_t k = std::min<size_t>(topster_size, n_docs);
+        if(filter_ids) k = std::min(k, filter_ids->size());
+        return (uint32_t) std::max<size_t>(1, k);
+    }
+    void size_topster(kw_query& q, size_t topster_size) const {
+        if(topster_size <= TSGPU_MAX_TOPK) { q.topk = (uint32_t) topster_size; return; }
+        q.topk = deep_topk(topster_size, q.has_filter ? &q.filter_ids : nullptr);
+        if(q.topk > TSGPU_MAX_TOPK) q.flags |= TSGPU_QFLAG_DEEP_TOPSTER;
+    }
+    // vector and hybrid queries: the fusion kernel holds the Topster in shared memory, so they stay at TSGPU_MAX_TOPK
+    static void clamp_topster(kw_query& q, size_t topster_size) {
+        q.topk = (uint32_t) std::min<size_t>(topster_size, TSGPU_MAX_TOPK);
+        q.flags &= (uint8_t) ~TSGPU_QFLAG_DEEP_TOPSTER;
     }
 
     // Keyword + vector query in ONE device call with reciprocal-rank fusion (Index::search with a vector_query,
@@ -739,6 +757,7 @@ public:
         kw_query q = make_kw_query(query_suggestions, 0, total_costs, the_fields, field_weights, sort_fields, filter_ids ? *filter_ids : std::vector<uint32_t>(),
                                    filter_ids != nullptr, excluded_result_ids, topster_size, o.prioritize_exact_match, o.prioritize_token_position,
                                    o.prioritize_num_matching_fields, o.text_match_type, -1, -1, false, false);
+        clamp_topster(q, topster_size);
         std::vector<kw_query*> one{&q};
         run_kw_batch(one, 2, query_vector, &vp);
         if(!q.status.ok()) return q.status;
@@ -753,6 +772,7 @@ public:
                                const tsgpu_vec_params& vp, std::vector<KV>& raw_result_kvs, size_t& found) {
         kw_query q = make_kw_query({}, 0, {}, {}, {}, sort_fields, filter_ids ? *filter_ids : std::vector<uint32_t>(), filter_ids != nullptr,
                                    excluded_result_ids, topster_size, true, false, true, TSGPU_MATCH_MAX_SCORE, -1, -1, false, false);
+        clamp_topster(q, topster_size);
         std::vector<kw_query*> one{&q};
         run_kw_batch(one, 1, query_vector, &vp);
         if(!q.status.ok()) return q.status;
@@ -891,7 +911,17 @@ public:
         kw_batch_storage(const kw_batch_storage&) = delete;
     };
     // what: 0 tsgpu_keyword_search_batch, 1 tsgpu_vector_search_batch, 2 tsgpu_hybrid_search_batch (qvecs: one vector per query)
+    // A deep query (TSGPU_QFLAG_DEEP_TOPSTER) goes to the device in a call of its own: the call's kv_stride is its widest Topster.
     void run_kw_batch(const std::vector<kw_query*>& qs, int what = 0, const float* qvecs = nullptr, const tsgpu_vec_params* vp = nullptr) {
+        if(qs.size() > 1 && std::any_of(qs.begin(), qs.end(), [](const kw_query* q) { return (q->flags & TSGPU_QFLAG_DEEP_TOPSTER) != 0; })) {
+            std::vector<kw_query*> rest;
+            for(kw_query* q: qs) {
+                if(q->flags & TSGPU_QFLAG_DEEP_TOPSTER) run_kw_batch(std::vector<kw_query*>{q}, what, qvecs, vp);
+                else rest.push_back(q);
+            }
+            if(!rest.empty()) run_kw_batch(rest, what, qvecs, vp);
+            return;
+        }
         kw_batch_storage st(qs);
         const uint32_t nq = (uint32_t) qs.size(), stride = st.stride;
         staged<KV> kvs(staging, (size_t) nq * stride);
@@ -1165,7 +1195,7 @@ public:
         uint32_t q_combo_off[2] = {0, 0};
         int32_t q_filter = filter_ids ? 0 : -1;
         uint32_t q_excl_off[2] = {0, (uint32_t) excluded_result_ids.size()};
-        uint32_t q_topk = (uint32_t) std::min<size_t>(topster_size, TSGPU_MAX_TOPK);
+        const uint32_t q_topk = topster_size <= TSGPU_MAX_TOPK ? (uint32_t) topster_size : deep_topk(topster_size, filter_ids);
         uint8_t sort_type[3] = {0, 0, 0}, missing_first[3] = {0, 0, 0};
         int32_t sort_col[3] = {-1, -1, -1};
         int8_t sort_order[3] = {1, 1, 1};
@@ -1175,7 +1205,7 @@ public:
             missing_first[i] = sort_fields[i].missing_first;
             if(sort_fields[i].type == sort_by::numeric) sort_col[i] = (int32_t) sort_cols.at(sort_fields[i].name);
         }
-        uint8_t q_flags = 0, q_match_type = TSGPU_MATCH_MAX_SCORE, q_nqt = 0, weight = 0;
+        uint8_t q_flags = q_topk > TSGPU_MAX_TOPK ? TSGPU_QFLAG_DEEP_TOPSTER : 0, q_match_type = TSGPU_MATCH_MAX_SCORE, q_nqt = 0, weight = 0;
         uint64_t filter_off[2] = {0, filter_ids ? filter_ids->size() : 0};
         const uint32_t zero = 0;
         uint32_t c_tok_off[1] = {0};
@@ -1884,8 +1914,11 @@ public:
             r.next = 0; r.cand_next = 0; r.has_pending = false; r.pending_walks.clear();
             replay() = &r;
             const auto& q = requests[i].r;
+            // the keyword stage of a hybrid request feeds tsgpu_hybrid_fuse_batch, whose Topster holds TSGPU_MAX_TOPK: all of it
+            // (token rounds, q=*, phrase-only, the host Topsters) stays at that size
+            const size_t topster_size = requests[i].query_vector ? std::min<size_t>(q.topster_size, TSGPU_MAX_TOPK) : q.topster_size;
             try {
-                out[i].status = search(q.tokens, q.the_fields, q.sort_fields, q.drop_tokens_threshold, q.topster_size, out[i].raw_result_kvs, out[i].found, q.opts);
+                out[i].status = search(q.tokens, q.the_fields, q.sort_fields, q.drop_tokens_threshold, topster_size, out[i].raw_result_kvs, out[i].found, q.opts);
                 done[i] = 1;
             }
             catch(const replay_suspend&) {}
@@ -1974,6 +2007,7 @@ public:
                 const std::vector<uint8_t> w = process_search_field_weights(rq.the_fields.size(), rq.opts.query_by_weights);
                 qv[k] = make_kw_query({}, 0, {}, rq.the_fields, w, rq.sort_fields, {}, false, {}, rq.topster_size, rq.opts.prioritize_exact_match,
                                       rq.opts.prioritize_token_position, rq.opts.prioritize_num_matching_fields, rq.opts.text_match_type, -1, -1, false, false);
+                clamp_topster(qv[k], rq.topster_size);
                 append_combos(qv[k], rs[i].executed);
                 qv[k].nqt = (uint8_t) rq.tokens.size();
                 qv[k].filter_handle = requests[i].filter_handle;

@@ -19,6 +19,9 @@ from .structs import KV_DTYPE
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 LIB_GPU = os.path.join(HERE, "libtshost.so")
+# tsgpu_kw_batch::q_flags bit the host layer sets when a keyword, wildcard or phrase-only search's topster_size exceeds
+# capi.MAX_TOPK (deep pagination); vector and hybrid searches stay at MAX_TOPK
+QFLAG_DEEP_TOPSTER = capi.QFLAG_DEEP_TOPSTER
 
 
 def build_gpu_lib(force: bool = False) -> str:

@@ -19,6 +19,8 @@ SORT_NONE, SORT_TEXT_MATCH, SORT_SEQ_ID, SORT_NUMERIC, SORT_VECTOR_DISTANCE = 0,
 MATCH_MAX_SCORE, MATCH_MAX_WEIGHT, MATCH_SUM_SCORE = 0, 1, 2
 FLAG_PRIORITIZE_EXACT_MATCH, FLAG_PRIORITIZE_TOKEN_POSITION, FLAG_PRIORITIZE_NUM_MATCHING_FIELDS = 1, 2, 4
 FLAG_RERANK_HYBRID_MATCHES, FLAG_KEEP_ALL_IDS = 0x40, 0x80
+FLAG_DEEP_TOPSTER = 0x20                  # q_topk may exceed MAX_TOPK (keyword, wildcard and scored-ids searches)
+MAX_TOPK = 1024
 CFLAG_SYNONYM, CFLAG_DEMOTE_SYNONYM = 1, 2
 
 u8p, u16p, u32p, u64p = (C.POINTER(C.c_uint8), C.POINTER(C.c_uint16), C.POINTER(C.c_uint32), C.POINTER(C.c_uint64))
@@ -76,7 +78,9 @@ class StatsStruct(C.Structure):
                 ("knn_expanded", C.c_uint64), ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64),
                 ("ms_kw_search", C.c_float), ("ms_kw_merge", C.c_float), ("ms_host_plan", C.c_float), ("knn_spec_hits", C.c_uint64),
                 ("knn_tier2_walks", C.c_uint64), ("knn_retried", C.c_uint64), ("h2d_total", C.c_uint64), ("d2h_total", C.c_uint64),
-                ("calls_total", C.c_uint64), ("knn_table_probes", C.c_uint64), ("flat_tc_queries", C.c_uint64)]
+                ("calls_total", C.c_uint64), ("knn_table_probes", C.c_uint64), ("flat_tc_queries", C.c_uint64),
+                ("deep_entries", C.c_uint64), ("deep_bytes", C.c_uint64), ("ms_deep_emit", C.c_float), ("ms_deep_dedup", C.c_float),
+                ("ms_deep_select", C.c_float), ("pad_deep", C.c_float)]
 
 
 def _ptr(a: Optional[np.ndarray], typ):
