@@ -422,6 +422,33 @@ tsgpu_status tsgpu_facet_counts_last(tsgpu_index* idx, uint32_t facet, uint32_t 
 /* all_result_ids of query q of the last search (ascending; needs TSGPU_QFLAG_KEEP_ALL_IDS). */
 tsgpu_status tsgpu_all_result_ids_last(tsgpu_index* idx, uint32_t q, uint32_t* out_ids, size_t cap, size_t* out_n);
 
+/* ---- diversity re-ranking ------------------------------------------------------------------------------------------ */
+/* One term of a curation rule's `diversity.similarity_metric` (include/diversity.h similarity_metric_t), resolved to the mirror. */
+enum { TSGPU_DIV_EQUALITY = 0, TSGPU_DIV_JACCARD = 1 };
+#define TSGPU_MAX_DIV_METRICS 16
+typedef struct {
+    uint32_t facet;      /* id from tsgpu_index_load_facet, or TSGPU_NO_LIST: use sort_col */
+    int32_t  sort_col;   /* sort column (tsgpu_index_load_sort_column) when facet == TSGPU_NO_LIST */
+    uint32_t method;     /* TSGPU_DIV_* */
+    float    weight;     /* 1 by default */
+} tsgpu_div_metric;
+/* Index::populate_result_kvs, diversity branch (src/index.cpp:9016-9064; similarity_t::calculate, src/diversity.cpp), batched:
+ * query q's records kv[q*kv_stride .. + count[q]] (a Topster after sort(), unique keys) are written to out_kv[q*kv_stride ..] in
+ * MMR order; the records themselves are unchanged. kv / out_kv: host or device memory (out_kv may be kv); lambda / count: host
+ * memory. lambda[q] in [0, 1]. Position 0 stays first; each next pick is the unpicked record with the greatest
+ * lambda * vector_distance - (1 - lambda) * (max similarity to the picked ones), the lowest position on a tie. Similarity sums the
+ * metrics in list order: a facet metric compares the two documents' facet values as sets (jaccard: |∩| / |∪| * weight; equality:
+ * weight when the sets are equal), a sort metric adds weight when both documents have a value and the values are equal (equality
+ * only); a document without values (an empty facet row, INT64_MIN, a seq_id >= the capacity) adds nothing. Arithmetic in the
+ * reference's float / double types, so the order is the reference's bit for bit. An unknown facet id or sort column, a method
+ * outside the enum, n_metrics == 0, count[q] > kv_stride or a lambda that is NaN or outside [0, 1] is TSGPU_ERR_INVALID;
+ * n_metrics > TSGPU_MAX_DIV_METRICS or a device scratch that cannot be allocated is TSGPU_ERR_CAPACITY (the message gives the
+ * bytes); the index stays usable. tsgpu_get_stats afterwards: ms_kernels = device time of the kernels, ms_total = the whole
+ * call on the stream. */
+tsgpu_status tsgpu_diversify_batch(tsgpu_index* idx, const tsgpu_div_metric* metrics, uint32_t n_metrics, uint32_t nq,
+                                   const float* lambda, const tsgpu_kv* kv, uint32_t kv_stride, const uint32_t* count,
+                                   tsgpu_kv* out_kv);
+
 /* ---- instrumentation ------------------------------------------------------------------------------------------ */
 /* Device-time breakdown of the last search call on this index (CUDA events on the library's stream), kernel launch
  * count since index creation, and algorithmic work counters of the last call. */

@@ -22,7 +22,7 @@ EXPORTS = [
     "tsgpu_index_load_sort_column", "tsgpu_index_append_lists", "tsgpu_index_set_sort_values", "tsgpu_index_load_hnsw", "tsgpu_index_build_hnsw", "tsgpu_index_append_hnsw", "tsgpu_index_mark_deleted", "tsgpu_index_hnsw_info", "tsgpu_index_export_hnsw", "tsgpu_filter_create", "tsgpu_filter_destroy", "tsgpu_filter_numeric", "tsgpu_filter_combine", "tsgpu_filter_ids", "tsgpu_scored_ids_search_batch",
     "tsgpu_intersect", "tsgpu_contains_atleast_one", "tsgpu_phrase_matches", "tsgpu_exact_matches", "tsgpu_prefix_matches", "tsgpu_ids_setop", "tsgpu_keyword_search_batch", "tsgpu_wildcard_search_batch", "tsgpu_knn_batch", "tsgpu_flat_distances", "tsgpu_flat_distances_batch",
     "tsgpu_vector_search_batch", "tsgpu_hybrid_search_batch", "tsgpu_get_stats", "tsgpu_debug_knn_work", "tsgpu_comm_unique_id", "tsgpu_comm_init", "tsgpu_comm_destroy", "tsgpu_comm_gather", "tsgpu_comm_last_ms", "tsgpu_hybrid_fuse_batch", "tsgpu_index_load_facet", "tsgpu_facet_counts", "tsgpu_facet_counts_last", "tsgpu_all_result_ids_last", "tsgpu_index_load_art", "tsgpu_art_walk_batch",
-    "tsgpu_index_compact_field", "tsgpu_index_reserve_docs", "tsgpu_index_field_info", "tsgpu_debug_field_array",
+    "tsgpu_index_compact_field", "tsgpu_index_reserve_docs", "tsgpu_index_field_info", "tsgpu_debug_field_array", "tsgpu_diversify_batch",
 ]
 
 
@@ -32,6 +32,14 @@ class FieldInfoStruct(C.Structure):
                 ("n_words", C.c_uint64), ("n_dense", C.c_uint32), ("dense_words", C.c_uint32), ("device_bytes", C.c_uint64)]
 
 
+class DivMetricStruct(C.Structure):
+    """tsgpu_div_metric: facet id (NO_LIST: use sort_col), sort column, TSGPU_DIV_* method, weight"""
+    _fields_ = [("facet", C.c_uint32), ("sort_col", C.c_int32), ("method", C.c_uint32), ("weight", C.c_float)]
+
+
+NO_LIST = 0xFFFFFFFF
+DIV_EQUALITY, DIV_JACCARD = 0, 1
+MAX_DIV_METRICS = 16
 FIELD_IS_ARRAY, FIELD_PLAIN_OK, FIELD_POS16 = 1, 2, 4
 # tsgpu_debug_field_array slots: name and element type
 FIELD_ARRAYS = [("list_off", np.uint64), ("list_blk_off", np.uint32), ("blk_first", np.uint32), ("blk_info", np.uint64), ("packed", np.uint32),
@@ -78,6 +86,9 @@ def declare(L):
                            ("tsgpu_debug_field_array", [vp, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)])):
             if hasattr(L, name):
                 getattr(L, name).argtypes = args
+        if hasattr(L, "tsgpu_diversify_batch"):      # absent from the base test double
+            L.tsgpu_diversify_batch.argtypes = [vp, C.POINTER(DivMetricStruct), C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32,
+                                                C.c_void_p, C.c_void_p]
         L.tsgpu_index_load_hnsw.argtypes = [vp, C.POINTER(HnswStruct)]
         L.tsgpu_index_build_hnsw.argtypes = [vp, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int]
         L.tsgpu_index_append_hnsw.argtypes = [vp, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]
@@ -199,6 +210,23 @@ class GpuIndex:
         """tsgpu_index_reserve_docs: raise the seq_id capacity."""
         _ck(self.L.tsgpu_index_reserve_docs(self.h, n_docs))
         self.n_docs = n_docs
+
+    def diversify(self, metrics, lambdas, kv, count, out=None, stride=None):
+        """tsgpu_diversify_batch: each query's records kv[q, :count[q]] in MMR order. metrics: (facet id or None, sort column, method,
+        weight) tuples; lambdas: one per query. kv / out: numpy [nq, stride] KV_DTYPE arrays, or CUDA tensors holding such
+        records (then `stride` gives the records per row). Returns `out` (a new array when kv is a numpy array and out is None)."""
+        m = (DivMetricStruct * max(1, len(metrics)))()
+        for i, (facet, col, method, weight) in enumerate(metrics):
+            m[i].facet = NO_LIST if facet is None else facet
+            m[i].sort_col, m[i].method, m[i].weight = col, method, weight
+        cnt = np.ascontiguousarray(count, np.uint32)
+        lam = np.ascontiguousarray(lambdas, np.float32)
+        if isinstance(kv, np.ndarray):
+            stride = kv.shape[1]
+            if out is None:
+                out = np.zeros_like(kv)
+        _ck(self.L.tsgpu_diversify_batch(self.h, m, len(metrics), len(cnt), lam.ctypes.data, _addr(kv), stride, cnt.ctypes.data, _addr(out)))
+        return out
 
     def field_info(self, field: int) -> dict:
         s = FieldInfoStruct()

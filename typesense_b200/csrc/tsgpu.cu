@@ -24,6 +24,7 @@
 #include "facet_kernels.cuh"
 #include "mirror_kernels.cuh"
 #include "deep_topster.cuh"
+#include "diversity.cuh"
 #include "postings_pack.h"
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
@@ -43,6 +44,9 @@ extern "C" void tsgpu_art_release_(const tsgpu_index* idx);
 // kw_regscore.cu: kw_search_kernel<true> lives in its own translation unit (see there)
 extern "C" cudaError_t tsgpu_launch_kw_search_regscore(const void* index_dev, const void* kw_params, unsigned n_units, size_t smem, cudaStream_t st);
 extern "C" cudaError_t tsgpu_launch_kw_search_deep(const void* index_dev, const void* kw_params, unsigned n_units, size_t smem, cudaStream_t st);
+// diversity.cu: the MMR re-ranking kernels (tsgpu_diversify_batch)
+extern "C" cudaError_t tsgpu_launch_div_count_(const tsdiv::Params* P, unsigned nq, cudaStream_t st);
+extern "C" cudaError_t tsgpu_launch_div_mmr_(const tsdiv::Params* P, unsigned nq, size_t smem, cudaStream_t st);
 
 namespace {
 
@@ -161,6 +165,8 @@ struct tsgpu_index {
     bool found_dirty = false;            // d_found_bm is all-zero between calls unless a call died before its popcount pass
     cudaEvent_t ev[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     cudaEvent_t deep_ev[4] = {nullptr, nullptr, nullptr, nullptr};     // emit / de-duplicate / select of deep queries (created on first use)
+    DevBuf d_div, d_div_ws;              // tsgpu_diversify_batch: records, per-query arrays / the workspaces that do not fit in shared memory
+    PinBuf h_div;
     tsgpu_stats stats{};
 };
 
@@ -1248,6 +1254,7 @@ void tsgpu_index_destroy(tsgpu_index* idx) {
     DevBuf* bufs[] = {&idx->d_stage, &idx->d_pool, &idx->d_small, &idx->d_bitmaps, &idx->d_found_bm, &idx->d_out, &idx->d_knn_vis,
                       &idx->d_knn_retry_vis, &idx->d_knn_retry_cand, &idx->d_knn_cand, &idx->d_knn_out, &idx->d_isect, &idx->d_kw_out, &idx->d_deep};
     for(auto* b: bufs) b->release();
+    idx->d_div.release(); idx->d_div_ws.release(); idx->h_div.release();
     idx->h_stage.release();
     for(auto& e: idx->ev) if(e) cudaEventDestroy(e);
     for(auto& e: idx->deep_ev) if(e) cudaEventDestroy(e);
@@ -1554,6 +1561,7 @@ tsgpu_status tsgpu_index_load_hnsw(tsgpu_index* idx, const tsgpu_hnsw* g) {
 #include "facet_host.inc"
 #include "comm_host.inc"
 #include "mirror_host.inc"
+#include "diversity_host.inc"
 
 tsgpu_status tsgpu_filter_create(tsgpu_index* idx, const uint32_t* ids, size_t n, int32_t* out_handle) {
     tsgpu_status s = check_device(idx); if(s) return s;

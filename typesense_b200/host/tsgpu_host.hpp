@@ -51,6 +51,10 @@
 #include "../../include/tsgpu.h"
 #include "art_mirror.hpp"
 
+// tsgpu_diversify_batch is referenced weakly: a program linked against a C-ABI library without it (the oracle-backed test double
+// of the CPU arm) still links, and only a request that asks for diversity reports the missing call.
+#pragma weak tsgpu_diversify_batch
+
 namespace tsgpu {
 
 template <class T>
@@ -208,6 +212,14 @@ struct search_options {
     // The column holds the documents' distinct ids (INT64_MIN = no value), see Index::search_grouped.
     const std::vector<int64_t>* group_column = nullptr;
     bool group_missing_values = false;
+    // Diversity: a matched curation rule's `diversity.similarity_metric` list (src/collection.cpp:1095-1108) and the
+    // `diversity_lambda` search parameter (src/collection.cpp:8479, 8606-8614). With metrics, the request's final list is put in
+    // maximal-marginal-relevance order (Index::populate_result_kvs, src/index.cpp:9016-9064) on the device. A field is looked up
+    // among the facet fields (Index::add_facet_field) first, then the sort fields. search_grouped ignores the metrics, as the
+    // reference's group branch does.
+    struct diversity_metric { std::string field; int method = TSGPU_DIV_EQUALITY; float weight = 1.0f; };
+    std::vector<diversity_metric> diversity;
+    float diversity_lambda = 0.5f;
 };
 
 // Incremental optimal-string-alignment rows as src/art.cpp:1412-1433 computes them while it walks a key: rows[i][col] =
@@ -333,6 +345,7 @@ class Index {
     uint32_t n_docs;
     std::vector<std::unordered_map<std::string, uint32_t>> token_ids;      // per field: token -> posting list id (art_search stand-in)
     std::unordered_map<std::string, uint32_t> field_ids, sort_cols;
+    std::unordered_map<std::string, uint32_t> facet_fields;                // facet field name -> tsgpu_index_load_facet id
     // what the ART leaves carry for candidate ordering: per field token strings by list id, their document frequency and
     // ids (for max_score over the default sorting field)
     struct vocab_t { std::vector<std::string> tokens; std::vector<uint64_t> list_off; std::vector<uint32_t> ids; };
@@ -570,6 +583,19 @@ public:
         arts_ready.assign(arts_ready.size(), 0);
         if(default_sorting_field.empty()) default_sorting_field = name;
         return Option<uint32_t>(col);
+    }
+    // facet_index_t of one facet field (what diversity metrics compare): document d holds value_ids[doc_off[d] .. doc_off[d + 1]),
+    // the dense ids the reference assigns per distinct value; doc_off has n_docs + 1 entries
+    Option<uint32_t> add_facet_field(const std::string& name, const std::vector<uint64_t>& doc_off, const std::vector<uint32_t>& value_ids) {
+        if(doc_off.size() != (size_t) n_docs + 1 || doc_off.back() != value_ids.size()) return Option<uint32_t>(400, "doc_off must have n_docs + 1 entries ending at the value count");
+        uint32_t n_values = 0;
+        for(uint32_t v: value_ids) n_values = std::max(n_values, v + 1);
+        const uint32_t zero = 0;
+        const tsgpu_facet f{n_values, doc_off.data(), value_ids.empty() ? &zero : value_ids.data()};
+        uint32_t id = 0;
+        if(tsgpu_index_load_facet(h, &f, &id) != TSGPU_OK) return Option<uint32_t>(500, tsgpu_last_error());
+        facet_fields[name] = id;
+        return Option<uint32_t>(id);
     }
     Option<bool> add_vector_field(const tsgpu_hnsw& g) {
         if(tsgpu_index_load_hnsw(h, &g) != TSGPU_OK) return Option<bool>(500, tsgpu_last_error());
@@ -1563,10 +1589,79 @@ public:
     }
 
     // Index::search for already-tokenised text: fuzzy_search_fields on the whole query, then the drop-tokens loop
-    // (src/index.cpp:3920-4017, right_to_left first) while fewer than drop_tokens_threshold results exist.
+    // (src/index.cpp:3920-4017, right_to_left first) while fewer than drop_tokens_threshold results exist. With diversity metrics
+    // the final list is re-ranked (Index::populate_result_kvs), whichever path produced it.
     Option<bool> search(const std::vector<std::string>& tokens, const std::vector<std::string>& the_fields,
                         const std::vector<sort_by>& sort_fields, size_t drop_tokens_threshold, size_t topster_size,
                         std::vector<KV>& raw_result_kvs, size_t& found, const search_options& opts = search_options()) {
+        auto op = search_topster(tokens, the_fields, sort_fields, drop_tokens_threshold, topster_size, raw_result_kvs, found, opts);
+        if(!op.ok() || opts.diversity.empty()) return op;
+        std::vector<Option<bool>> status;
+        diversify_lists({&raw_result_kvs}, {&opts}, status);
+        return status[0];
+    }
+
+    // Index::populate_result_kvs, diversity branch (src/index.cpp:9016-9064), for several final lists at once: each list with
+    // metrics is put in MMR order, and lists that share a metric list go through one tsgpu_diversify_batch. A metric names a facet
+    // field, else a sort field, as similarity_t::calculate looks them up (src/diversity.cpp); any other name is the reference's
+    // 400, raised as there only when a pair is compared (a list of two or more). status[i]: the outcome for list i.
+    void diversify_lists(const std::vector<std::vector<KV>*>& lists, const std::vector<const search_options*>& opts, std::vector<Option<bool>>& status) {
+        status.assign(lists.size(), Option<bool>(true));
+        std::map<std::string, std::vector<size_t>> groups;                   // resolved metric list (bytes) -> lists
+        std::map<std::string, std::vector<tsgpu_div_metric>> metrics_of;
+        for(size_t i = 0; i < lists.size(); i++) {
+            if(opts[i]->diversity.empty() || lists[i]->size() < 2) continue;
+            std::vector<tsgpu_div_metric> m;
+            for(auto& dm: opts[i]->diversity) {
+                tsgpu_div_metric x{TSGPU_NO_LIST, -1, (uint32_t) dm.method, dm.weight};
+                auto f = facet_fields.find(dm.field);
+                auto c = sort_cols.find(dm.field);
+                if(f != facet_fields.end()) x.facet = f->second;
+                else if(c != sort_cols.end()) x.sort_col = (int32_t) c->second;
+                else { status[i] = Option<bool>(400, "`" + dm.field + "` field not found in either facet or sort index."); break; }
+                m.push_back(x);
+            }
+            if(!status[i].ok()) continue;
+            std::string key(reinterpret_cast<const char*>(m.data()), m.size() * sizeof(tsgpu_div_metric));
+            groups[key].push_back(i);
+            metrics_of[key] = std::move(m);
+        }
+        for(auto& g: groups) {
+            const auto& ids = g.second;
+            if(!tsgpu_diversify_batch) {
+                for(size_t i: ids) status[i] = Option<bool>(500, "the C-ABI library has no tsgpu_diversify_batch");
+                continue;
+            }
+            uint32_t stride = 1;
+            for(size_t i: ids) stride = std::max<uint32_t>(stride, (uint32_t) lists[i]->size());
+            std::vector<KV> kv((size_t) ids.size() * stride);
+            std::vector<uint32_t> count(ids.size());
+            std::vector<float> lambda(ids.size());
+            for(size_t k = 0; k < ids.size(); k++) {
+                std::copy(lists[ids[k]]->begin(), lists[ids[k]]->end(), kv.begin() + (ptrdiff_t) (k * stride));
+                count[k] = (uint32_t) lists[ids[k]]->size();
+                // the `diversity_lambda` parameter keeps its default unless the value is within [0, 1] (src/collection.cpp:8606-8614)
+                const float l = opts[ids[k]]->diversity_lambda;
+                lambda[k] = l >= 0.0f && l <= 1.0f ? l : 0.5f;
+            }
+            const auto& m = metrics_of[g.first];
+            const tsgpu_status rc = tsgpu_diversify_batch(h, m.data(), (uint32_t) m.size(), (uint32_t) ids.size(), lambda.data(), kv.data(), stride,
+                                                          count.data(), kv.data());
+            if(rc != TSGPU_OK) {
+                const Option<bool> e(rc == TSGPU_ERR_INVALID ? 400 : 500, tsgpu_last_error());
+                for(size_t i: ids) status[i] = e;
+                continue;
+            }
+            for(size_t k = 0; k < ids.size(); k++)
+                std::copy(kv.begin() + (ptrdiff_t) (k * stride), kv.begin() + (ptrdiff_t) (k * stride + count[k]), lists[ids[k]]->begin());
+        }
+    }
+
+    // Index::search up to the sorted Topster, before populate_result_kvs: what search() re-ranks, what search_grouped groups and
+    // what the keyword stage of a hybrid request hands to the rank fusion.
+    Option<bool> search_topster(const std::vector<std::string>& tokens, const std::vector<std::string>& the_fields,
+                                const std::vector<sort_by>& sort_fields, size_t drop_tokens_threshold, size_t topster_size,
+                                std::vector<KV>& raw_result_kvs, size_t& found, const search_options& opts) {
         search_state st(topster_size);
         st.weights = process_search_field_weights(the_fields.size(), opts.query_by_weights);
         auto xop = handle_exclusion(the_fields, opts, st.excluded);
@@ -1683,7 +1778,7 @@ public:
             Option<bool> op(true);
             search_options go = opts;
             go.group_column = &col; go.group_missing_values = group_missing_values;
-            try { op = search(tokens, the_fields, sort_fields, drop_tokens_threshold, T, kvs, found, go); }
+            try { op = search_topster(tokens, the_fields, sort_fields, drop_tokens_threshold, T, kvs, found, go); }
             catch(...) { round_recorder() = nullptr; throw; }
             round_recorder() = nullptr;
             if(!op.ok()) return op;
@@ -1918,7 +2013,7 @@ public:
             // (token rounds, q=*, phrase-only, the host Topsters) stays at that size
             const size_t topster_size = requests[i].query_vector ? std::min<size_t>(q.topster_size, TSGPU_MAX_TOPK) : q.topster_size;
             try {
-                out[i].status = search(q.tokens, q.the_fields, q.sort_fields, q.drop_tokens_threshold, topster_size, out[i].raw_result_kvs, out[i].found, q.opts);
+                out[i].status = search_topster(q.tokens, q.the_fields, q.sort_fields, q.drop_tokens_threshold, topster_size, out[i].raw_result_kvs, out[i].found, q.opts);
                 done[i] = 1;
             }
             catch(const replay_suspend&) {}
@@ -2027,6 +2122,10 @@ public:
             }
             uint32_t stride = 1;
             for(size_t i: ids) stride = std::max<uint32_t>(stride, (uint32_t) std::min<size_t>(requests[i].hits ? requests[i].hits : requests[i].r.topster_size, st.stride));
+            // a request with diversity metrics needs its whole fused Topster: MMR over a truncated list picks differently. The others
+            // keep the records they had without it (stride_hits).
+            const uint32_t stride_hits = stride;
+            for(size_t i: ids) if(!requests[i].r.opts.diversity.empty()) stride = std::max<uint32_t>(stride, (uint32_t) std::min<size_t>(requests[i].r.topster_size, st.stride));
             staged<KV> okv(staging, (size_t) m * stride);
             std::vector<uint32_t> ocount(m), ofound(m);
             const tsgpu_vec_params vp = requests[ids[0]].vp;
@@ -2038,11 +2137,30 @@ public:
             }
             bs.fuse_queries += m;
             for(size_t k = 0; k < m; k++) {
-                out[ids[k]].raw_result_kvs.assign(okv.data() + k * stride, okv.data() + k * stride + ocount[k]);
+                const uint32_t c = requests[ids[k]].r.opts.diversity.empty() ? std::min(ocount[k], stride_hits) : ocount[k];
+                out[ids[k]].raw_result_kvs.assign(okv.data() + k * stride, okv.data() + k * stride + c);
                 out[ids[k]].found = ofound[k];
             }
         }
         bs.ms_fuse_calls = ms_since(tfuse);
+        // ---- diversity: every final list with metrics (keyword, q=*, phrase-only and hybrid alike), one call per metric list; a
+        // hybrid request is cut to its `hits` only after the re-ranking
+        {
+            std::vector<std::vector<KV>*> lists;
+            std::vector<const search_options*> lopts;
+            std::vector<size_t> which;
+            for(size_t i = 0; i < n; i++) {
+                if(requests[i].r.opts.diversity.empty() || !out[i].status.ok()) continue;
+                lists.push_back(&out[i].raw_result_kvs); lopts.push_back(&requests[i].r.opts); which.push_back(i);
+            }
+            std::vector<Option<bool>> dst;
+            if(!lists.empty()) diversify_lists(lists, lopts, dst);
+            for(size_t k = 0; k < which.size(); k++) {
+                const size_t i = which[k];
+                out[i].status = dst[k];
+                if(requests[i].query_vector && requests[i].hits && out[i].raw_result_kvs.size() > requests[i].hits) out[i].raw_result_kvs.resize(requests[i].hits);
+            }
+        }
         if(stats) *stats = bs;
         return out;
     }
