@@ -141,6 +141,17 @@ typedef struct {
  * (see tsgpu_flat_distances_batch): same ids, distances within ~1e-6 absolute of the fp32 loop instead of bit-equal — so two
  * candidates whose distances differ by less than that may swap ranks. Opt-in for that reason. */
 #define TSGPU_VEC_FLAT_TENSOR 1u
+/* Deep pagination for vector and hybrid searches: with this bit tsgpu_vector_search_batch, tsgpu_hybrid_search_batch and
+ * tsgpu_hybrid_fuse_batch accept TSGPU_QFLAG_DEEP_TOPSTER with any q_topk >= 1, and the hybrid calls accept k up to the vector
+ * stage's bound max(ef, k) <= 4096 (above it TSGPU_ERR_CAPACITY, as for every vector call). A query with the flag and q_topk >
+ * TSGPU_MAX_TOPK is fused by the deep kernels (deep_fuse.cuh): the same answer as the reference at any Topster size, with a
+ * per-call device buffer sized by the request (vector: 32 bytes per kNN / flat result; hybrid: 69 bytes per Topster slot and
+ * 42 per vector result, both counts padded to a power of two, in shared memory when a query's workspace fits). When it cannot be allocated the call returns
+ * TSGPU_ERR_CAPACITY (the message gives the bytes) and the index stays usable; a buffer above 256 MiB is freed when the call
+ * returns. The other queries of the batch run the ordinary kernels, byte for byte as without the bit. Opt-in for the buffer's
+ * sake, as TSGPU_QFLAG_DEEP_TOPSTER is; composes with TSGPU_VEC_FLAT_TENSOR. kv_stride, out_found, query_index and
+ * TSGPU_QFLAG_KEEP_ALL_IDS keep their meaning. */
+#define TSGPU_VEC_DEEP_TOPSTER 2u
 
 const char* tsgpu_last_error(void);
 int tsgpu_device_count(void);
@@ -398,7 +409,8 @@ tsgpu_status tsgpu_comm_last_ms(tsgpu_index* idx, float* out_ms);     /* device 
  * flag changes nothing. Outputs keep their meaning: kv_stride truncates a query's records, out_found and query_index are
  * as without the flag. Honoured by tsgpu_keyword_search_batch, tsgpu_wildcard_search_batch and
  * tsgpu_scored_ids_search_batch; the vector and hybrid calls (tsgpu_vector_search_batch, tsgpu_hybrid_search_batch,
- * tsgpu_hybrid_fuse_batch) reject it with TSGPU_ERR_INVALID, since their fusion keeps the Topster in shared memory. */
+ * tsgpu_hybrid_fuse_batch) reject it with TSGPU_ERR_INVALID, since their fusion keeps the Topster in shared memory, unless
+ * tsgpu_vec_params::flags has TSGPU_VEC_DEEP_TOPSTER. */
 #define TSGPU_QFLAG_DEEP_TOPSTER 0x20u
 /* Mirror of one facet field: facet_index_t's seq_id -> facet ids (src/facet_index.cpp:27-90; ids are the dense counter the
  * reference assigns per distinct value; a binding densifies numeric facets the same way). Host or device pointers. */
@@ -483,6 +495,11 @@ typedef struct {
     float    ms_deep_dedup;      /* de-duplication of the deep queries' entries per seq_id */
     float    ms_deep_select;     /* sort of the distinct entries and the record write */
     float    pad_deep;
+    uint64_t deep_fuse_bytes;    /* device bytes of the deep vector / hybrid workspace of the last call (TSGPU_VEC_DEEP_TOPSTER) */
+    float    ms_deep_fuse_prep;  /* deep hybrid fusion, slowest deep query of each phase: keyword Topster, text ranks, vector list, */
+    float    ms_deep_fuse_replay;/*   per-result work | the serial replay of the loop | rerank_hybrid_matches | final sort and */
+    float    ms_deep_fuse_rerank;/*   write. Deep vector assembly: ms_deep_fuse_sort = the sorts and record writes */
+    float    ms_deep_fuse_sort;
 } tsgpu_stats;
 tsgpu_status tsgpu_get_stats(tsgpu_index* idx, tsgpu_stats* out);
 /* Instrumentation: per graph walk of the last HNSW launch, out[2q] = expanded nodes, out[2q+1] = distance evaluations. */

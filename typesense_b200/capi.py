@@ -48,6 +48,7 @@ FACET_DTYPE = np.dtype([("value_id", np.uint32), ("count", np.uint32), ("doc_id"
 QFLAG_KEEP_ALL_IDS = 0x80
 QFLAG_DEEP_TOPSTER = 0x20       # q_topk may exceed MAX_TOPK (tsgpu_keyword / wildcard / scored_ids_search_batch)
 MAX_TOPK = 1024
+VEC_DEEP_TOPSTER = 2            # tsgpu_vec_params::flags: the vector / hybrid calls accept QFLAG_DEEP_TOPSTER (deep fusion)
 
 
 class TsgpuError(RuntimeError):

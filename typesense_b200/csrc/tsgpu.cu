@@ -25,6 +25,7 @@
 #include "mirror_kernels.cuh"
 #include "deep_topster.cuh"
 #include "diversity.cuh"
+#include "deep_fuse.cuh"
 #include "postings_pack.h"
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
@@ -165,6 +166,7 @@ struct tsgpu_index {
     bool found_dirty = false;            // d_found_bm is all-zero between calls unless a call died before its popcount pass
     cudaEvent_t ev[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     cudaEvent_t deep_ev[4] = {nullptr, nullptr, nullptr, nullptr};     // emit / de-duplicate / select of deep queries (created on first use)
+    DevBuf d_fuse;                       // deep vector assembly / deep hybrid fusion (deep_fuse_host.inc)
     DevBuf d_div, d_div_ws;              // tsgpu_diversify_batch: records, per-query arrays / the workspaces that do not fit in shared memory
     PinBuf h_div;
     tsgpu_stats stats{};
@@ -1181,6 +1183,8 @@ tsgpu_status run_vector_stage(tsgpu_index* idx, const tsgpu_kw_batch* b, KwPlan&
     return run_knn(idx, reinterpret_cast<const float*>(base + o_q), nq, k, vp->ef, pl.q_bitmap, pl.q_excl_dev, nexcl, skip, cost, vs.knn);
 }
 
+#include "deep_fuse_host.inc"
+
 }  // namespace
 
 // ===================================================================================================== C API
@@ -1252,7 +1256,7 @@ void tsgpu_index_destroy(tsgpu_index* idx) {
     idx->d_keep_bm.release(); idx->d_facet.release(); idx->d_comm.release();
     if(idx->comm) { tsgpu_comm_destroy(idx); }
     DevBuf* bufs[] = {&idx->d_stage, &idx->d_pool, &idx->d_small, &idx->d_bitmaps, &idx->d_found_bm, &idx->d_out, &idx->d_knn_vis,
-                      &idx->d_knn_retry_vis, &idx->d_knn_retry_cand, &idx->d_knn_cand, &idx->d_knn_out, &idx->d_isect, &idx->d_kw_out, &idx->d_deep};
+                      &idx->d_knn_retry_vis, &idx->d_knn_retry_cand, &idx->d_knn_cand, &idx->d_knn_out, &idx->d_isect, &idx->d_kw_out, &idx->d_deep, &idx->d_fuse};
     for(auto* b: bufs) b->release();
     idx->d_div.release(); idx->d_div_ws.release(); idx->h_div.release();
     idx->h_stage.release();
@@ -2071,8 +2075,10 @@ static tsgpu_status vec_or_hybrid(tsgpu_index* idx, const tsgpu_kw_batch* b, con
     tsgpu_status s = check_device(idx); if(s) return s;
     if(!b || !qvecs || !vp || !out_kv || !out_count || !out_found || kv_stride == 0) return fail(TSGPU_ERR_INVALID, "null argument");
     if(!idx->has_hnsw) return fail(TSGPU_ERR_INVALID, "no vector index loaded");
-    for(uint32_t q = 0; q < b->n_queries; q++)         // the fusion kernel holds its Topster in shared memory
-        if(b->q_flags[q] & TSGPU_QFLAG_DEEP_TOPSTER) return fail(TSGPU_ERR_INVALID, "TSGPU_QFLAG_DEEP_TOPSTER is not supported by vector and hybrid searches");
+    const bool vdeep = (vp->flags & TSGPU_VEC_DEEP_TOPSTER) != 0;
+    if(!vdeep)
+        for(uint32_t q = 0; q < b->n_queries; q++)     // the ordinary fusion kernel holds its Topster in shared memory
+            if(b->q_flags[q] & TSGPU_QFLAG_DEEP_TOPSTER) return fail(TSGPU_ERR_INVALID, "TSGPU_QFLAG_DEEP_TOPSTER is not supported by vector and hybrid searches");
     std::lock_guard<std::mutex> lk(idx->mu);
     begin_call(idx);
     KwPlan pl;
@@ -2081,15 +2087,20 @@ static tsgpu_status vec_or_hybrid(tsgpu_index* idx, const tsgpu_kw_batch* b, con
       idx->stats.ms_host_plan = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count(); }
     if(s) return s;
     if(pl.nq == 0) return end_call(idx, false, false);
-    s = upload_kw_plan(idx, b, pl); if(s) return s;
-    cudaStream_t st = idx->stream;
-    const uint32_t nq = pl.nq;
-    KwDeviceOut kwo{};
     // k as in src/index.cpp:3646 (wildcard) and :4061-4063 (hybrid)
     const uint32_t k = hybrid ? (vp->k == 0 ? std::max<uint32_t>(vp->fetch_size, 100) : vp->k)
                               : (vp->k == 0 ? std::max<uint32_t>(vp->k, vp->fetch_size) : vp->k);
     if(k == 0) return fail(TSGPU_ERR_INVALID, "k resolves to 0 (set k or fetch_size)");
-    if(hybrid && k > 1024) return fail(TSGPU_ERR_CAPACITY, "hybrid k must be <= 1024");
+    if(hybrid && k > 1024 && !vdeep) return fail(TSGPU_ERR_CAPACITY, "hybrid k must be <= 1024");
+    // deep queries (TSGPU_VEC_DEEP_TOPSTER): planned and their device memory reserved before anything runs
+    DeepFuse df;
+    if(vdeep) { s = deep_fuse_plan(idx, b, pl, vp, k, hybrid, df); if(s) return s; }
+    s = upload_kw_plan(idx, b, pl); if(s) return s;
+    s = deep_fuse_upload(idx, pl, b, vp, k, df); if(s) return s;
+    cudaStream_t st = idx->stream;
+    const uint32_t nq = pl.nq;
+    KwDeviceOut kwo{};
+    const uint32_t kw_stride = std::max(std::max(kv_stride, pl.KMAX), df.kmax);     // a deep query's keyword Topster is whole
     // The vector stage and the keyword kernels are independent until the fusion: issue the vector stage on its own
     // stream (after the filter bitmaps built by upload_kw_plan) with a reduced residency so keyword CTAs co-run, and
     // let the long latency-bound tail of the graph walk hide under the keyword kernels.
@@ -2120,11 +2131,11 @@ static tsgpu_status vec_or_hybrid(tsgpu_index* idx, const tsgpu_kw_batch* b, con
         idx->stats.h2d_bytes += kvb + (size_t) nq * 12;
         CU(cudaEventRecord(idx->ev[1], st)); CU(cudaEventRecord(idx->ev[6], st)); CU(cudaEventRecord(idx->ev[2], st));
     }
-    else if(hybrid && kw_first) { s = run_keyword(idx, pl, std::max(kv_stride, pl.KMAX), kwo); if(s) return s; }
+    else if(hybrid && kw_first) { s = run_keyword(idx, pl, kw_stride, kwo); if(s) return s; }
     s = run_vector_stage(idx, b, pl, qvecs, vp, k, vs); if(s) return s;
     if(hybrid) {
         CU(cudaEventRecord(idx->evB, idx->stream2));
-        if(!kw_first && !given) { s = run_keyword(idx, pl, std::max(kv_stride, pl.KMAX), kwo); if(s) return s; }
+        if(!kw_first && !given) { s = run_keyword(idx, pl, kw_stride, kwo); if(s) return s; }
         CU(cudaStreamWaitEvent(st, idx->evB, 0));
     }
     // final assembly
@@ -2140,17 +2151,23 @@ static tsgpu_status vec_or_hybrid(tsgpu_index* idx, const tsgpu_kw_batch* b, con
     if(!hybrid) {
         tsf::VecAssembleParams P{};
         P.qd = pl.d_qd;
+        if(!df.q.empty()) {
+            s = deep_fuse_counts(idx, pl, nullptr, vs.knn.n, df); if(s) return s;
+            P.qd = df.d_qd_ord;
+        }
         P.res_dist = vs.knn.dist; P.res_ids = vs.knn.labels; P.res_n = vs.knn.n; P.res_stride = vs.knn.stride;
         P.flat_dist = vs.flat_dist; P.flat_ids = vs.flat_ids;
         P.res_off = vs.flat_off; P.q_is_flat = vs.any_flat ? vs.d_is_flat : nullptr;
         P.vp = dvp;
         P.out_kv = d_kv; P.out_count = d_cnt; P.out_found = d_found; P.kv_stride = kv_stride;
+        if(!df.q.empty()) P.res_n = df.d_res_n_ord;
         P.KP = std::max<uint32_t>(pl.KP, 256);          // 256 threads append per round
         const size_t smem = (size_t) 2 * P.KP * 32 + 16;
         CU(cudaFuncSetAttribute(tsf::vec_assemble_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) std::max<size_t>(smem, 48 * 1024)));
         tsf::vec_assemble_kernel<<<nq, kFinalThreads, smem, st>>>(P);
         idx->stats.launches_total++;
         CU(cudaGetLastError());
+        if(!df.q.empty()) { s = run_vec_deep(idx, pl, vs, dvp, df, d_kv, kv_stride, d_cnt, d_found); if(s) return s; }
     } else {
         tsf::HybridParams P{};
         P.ix = idx->ixdev; P.qd = pl.d_qd; P.cd = pl.d_cd; P.F = pl.F;
@@ -2166,9 +2183,15 @@ static tsgpu_status vec_or_hybrid(tsgpu_index* idx, const tsgpu_kw_batch* b, con
         const uint32_t KP2 = pow2_ceil(pl.KMAX), VP2 = pow2_ceil(k);
         const size_t smem = (size_t) pl.KMAX * sizeof(KVOut) + (size_t) (KP2 + 2) * 2 + (size_t) VP2 * (12 + 24 + 2) + 48;
         CU(cudaFuncSetAttribute(tsf::hybrid_fuse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) std::max<size_t>(smem, 48 * 1024)));
+        const tsf::HybridParams whole = P;
+        if(!df.q.empty()) {
+            s = deep_fuse_counts(idx, pl, kwo.count, vs.knn.n, df); if(s) return s;
+            P.qd = df.d_qd_ord; P.kw_count = df.d_kw_count_ord; P.res_n = df.d_res_n_ord;
+        }
         tsf::hybrid_fuse_kernel<<<nq, kThreads, smem, st>>>(P);
         idx->stats.launches_total++;
         CU(cudaGetLastError());
+        if(!df.q.empty()) { s = run_hybrid_deep(idx, whole, df); if(s) return s; }
     }
     cudaEventRecord(e1, st);
     CU(cudaMemcpyAsync(out_kv, d_kv, kv_bytes, cudaMemcpyDefault, st));
@@ -2177,6 +2200,7 @@ static tsgpu_status vec_or_hybrid(tsgpu_index* idx, const tsgpu_kw_batch* b, con
     idx->stats.d2h_bytes += kv_bytes + (size_t) nq * 8;
     s = end_call(idx, hybrid, true);
     if(!s) s = finish_knn(idx);
+    deep_fuse_finish(idx, hybrid, df);
     float ms = 0;
     cudaEventElapsedTime(&ms, e0, e1);
     idx->stats.ms_fuse = ms; idx->stats.ms_kernels += ms;

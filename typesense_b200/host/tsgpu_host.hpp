@@ -765,10 +765,15 @@ public:
         q.topk = deep_topk(topster_size, q.has_filter ? &q.filter_ids : nullptr);
         if(q.topk > TSGPU_MAX_TOPK) q.flags |= TSGPU_QFLAG_DEEP_TOPSTER;
     }
-    // vector and hybrid queries: the fusion kernel holds the Topster in shared memory, so they stay at TSGPU_MAX_TOPK
+    // vector and hybrid queries: the ordinary fusion kernel holds the Topster in shared memory, so without
+    // TSGPU_VEC_DEEP_TOPSTER they stay at TSGPU_MAX_TOPK; with it they are sized as keyword queries are (the deep fusion)
     static void clamp_topster(kw_query& q, size_t topster_size) {
         q.topk = (uint32_t) std::min<size_t>(topster_size, TSGPU_MAX_TOPK);
         q.flags &= (uint8_t) ~TSGPU_QFLAG_DEEP_TOPSTER;
+    }
+    void size_vec_topster(kw_query& q, size_t topster_size, const tsgpu_vec_params& vp) const {
+        if(vp.flags & TSGPU_VEC_DEEP_TOPSTER) size_topster(q, topster_size);
+        else clamp_topster(q, topster_size);
     }
 
     // Keyword + vector query in ONE device call with reciprocal-rank fusion (Index::search with a vector_query,
@@ -783,7 +788,7 @@ public:
         kw_query q = make_kw_query(query_suggestions, 0, total_costs, the_fields, field_weights, sort_fields, filter_ids ? *filter_ids : std::vector<uint32_t>(),
                                    filter_ids != nullptr, excluded_result_ids, topster_size, o.prioritize_exact_match, o.prioritize_token_position,
                                    o.prioritize_num_matching_fields, o.text_match_type, -1, -1, false, false);
-        clamp_topster(q, topster_size);
+        size_vec_topster(q, topster_size, vp);
         std::vector<kw_query*> one{&q};
         run_kw_batch(one, 2, query_vector, &vp);
         if(!q.status.ok()) return q.status;
@@ -798,7 +803,7 @@ public:
                                const tsgpu_vec_params& vp, std::vector<KV>& raw_result_kvs, size_t& found) {
         kw_query q = make_kw_query({}, 0, {}, {}, {}, sort_fields, filter_ids ? *filter_ids : std::vector<uint32_t>(), filter_ids != nullptr,
                                    excluded_result_ids, topster_size, true, false, true, TSGPU_MATCH_MAX_SCORE, -1, -1, false, false);
-        clamp_topster(q, topster_size);
+        size_vec_topster(q, topster_size, vp);
         std::vector<kw_query*> one{&q};
         run_kw_batch(one, 1, query_vector, &vp);
         if(!q.status.ok()) return q.status;
@@ -2009,9 +2014,11 @@ public:
             r.next = 0; r.cand_next = 0; r.has_pending = false; r.pending_walks.clear();
             replay() = &r;
             const auto& q = requests[i].r;
-            // the keyword stage of a hybrid request feeds tsgpu_hybrid_fuse_batch, whose Topster holds TSGPU_MAX_TOPK: all of it
-            // (token rounds, q=*, phrase-only, the host Topsters) stays at that size
-            const size_t topster_size = requests[i].query_vector ? std::min<size_t>(q.topster_size, TSGPU_MAX_TOPK) : q.topster_size;
+            // the keyword stage of a hybrid request feeds tsgpu_hybrid_fuse_batch, whose ordinary Topster holds TSGPU_MAX_TOPK: all
+            // of it (token rounds, q=*, phrase-only, the host Topsters) stays at that size unless the request asks for the deep
+            // fusion (TSGPU_VEC_DEEP_TOPSTER), which takes the whole keyword Topster
+            const bool deep_vec = (requests[i].vp.flags & TSGPU_VEC_DEEP_TOPSTER) != 0;
+            const size_t topster_size = requests[i].query_vector && !deep_vec ? std::min<size_t>(q.topster_size, TSGPU_MAX_TOPK) : q.topster_size;
             try {
                 out[i].status = search_topster(q.tokens, q.the_fields, q.sort_fields, q.drop_tokens_threshold, topster_size, out[i].raw_result_kvs, out[i].found, q.opts);
                 done[i] = 1;
@@ -2078,11 +2085,12 @@ public:
         auto tfuse = clk::now();
         std::vector<size_t> hyb;
         for(size_t i = 0; i < n; i++) if(requests[i].query_vector && out[i].status.ok()) hyb.push_back(i);
-        std::map<std::vector<uint32_t>, std::vector<size_t>> hgroups;        // same searched fields, same vector parameters per call
+        // same searched fields and the same TSGPU_VEC_DEEP_TOPSTER bit per call (a call takes one tsgpu_vec_params)
+        std::map<std::pair<std::vector<uint32_t>, uint32_t>, std::vector<size_t>> hgroups;
         for(size_t i: hyb) {
             std::vector<uint32_t> key = rs[i].executed.fids;
             if(key.empty()) for(auto& fn: requests[i].r.the_fields) key.push_back(field_ids.at(fn));
-            hgroups[key].push_back(i);
+            hgroups[{key, requests[i].vp.flags & TSGPU_VEC_DEEP_TOPSTER}].push_back(i);
         }
         for(auto& g: hgroups) {
             const auto& ids = g.second;
@@ -2102,7 +2110,7 @@ public:
                 const std::vector<uint8_t> w = process_search_field_weights(rq.the_fields.size(), rq.opts.query_by_weights);
                 qv[k] = make_kw_query({}, 0, {}, rq.the_fields, w, rq.sort_fields, {}, false, {}, rq.topster_size, rq.opts.prioritize_exact_match,
                                       rq.opts.prioritize_token_position, rq.opts.prioritize_num_matching_fields, rq.opts.text_match_type, -1, -1, false, false);
-                clamp_topster(qv[k], rq.topster_size);
+                size_vec_topster(qv[k], rq.topster_size, requests[i].vp);
                 append_combos(qv[k], rs[i].executed);
                 qv[k].nqt = (uint8_t) rq.tokens.size();
                 qv[k].filter_handle = requests[i].filter_handle;

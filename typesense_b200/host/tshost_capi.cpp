@@ -72,6 +72,7 @@ typedef struct {
     uint32_t num_typos, prefix, max_candidates, typo_tokens_threshold, drop_tokens_threshold, topster_size, device_art_walk, n_threads;
     uint32_t vec_k, vec_ef, vec_flat_search_cutoff, vec_fetch_size;
     float vec_alpha, vec_distance_threshold;
+    uint32_t vec_flags;          /* tsgpu_vec_params::flags of the vector requests (TSGPU_VEC_DEEP_TOPSTER: Topsters above 1024) */
 } tshost_options;
 typedef struct { uint64_t passes, kw_batches, kw_queries, walk_batches, walks, host_walk_fallbacks, fuse_queries; double ms_host_passes, ms_kw_calls, ms_walk_calls, ms_fuse_calls; } tshost_stats;
 
@@ -98,7 +99,7 @@ int tshost_multi_search(void* h, const char* field, const char* sort_field, uint
         reqs[i].hits = stride;
         if(qvecs) {
             reqs[i].query_vector = qvecs + (size_t) i * dim;
-            reqs[i].vp = tsgpu_vec_params{o->vec_k, o->vec_ef, o->vec_flat_search_cutoff, o->vec_distance_threshold, o->vec_alpha, o->vec_fetch_size, 0u};
+            reqs[i].vp = tsgpu_vec_params{o->vec_k, o->vec_ef, o->vec_flat_search_cutoff, o->vec_distance_threshold, o->vec_alpha, o->vec_fetch_size, o->vec_flags};
         }
     }
     Ix::batched_stats bs;

@@ -20,8 +20,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 LIB_GPU = os.path.join(HERE, "libtshost.so")
 # tsgpu_kw_batch::q_flags bit the host layer sets when a keyword, wildcard or phrase-only search's topster_size exceeds
-# capi.MAX_TOPK (deep pagination); vector and hybrid searches stay at MAX_TOPK
+# capi.MAX_TOPK (deep pagination); vector and hybrid searches stay at MAX_TOPK unless Options.vec_flags has VEC_DEEP_TOPSTER
 QFLAG_DEEP_TOPSTER = capi.QFLAG_DEEP_TOPSTER
+VEC_DEEP_TOPSTER = capi.VEC_DEEP_TOPSTER
 
 
 def build_gpu_lib(force: bool = False) -> str:
@@ -40,11 +41,12 @@ class Options(C.Structure):
     _fields_ = [("num_typos", C.c_uint32), ("prefix", C.c_uint32), ("max_candidates", C.c_uint32), ("typo_tokens_threshold", C.c_uint32),
                 ("drop_tokens_threshold", C.c_uint32), ("topster_size", C.c_uint32), ("device_art_walk", C.c_uint32), ("n_threads", C.c_uint32),
                 ("vec_k", C.c_uint32), ("vec_ef", C.c_uint32), ("vec_flat_search_cutoff", C.c_uint32), ("vec_fetch_size", C.c_uint32),
-                ("vec_alpha", C.c_float), ("vec_distance_threshold", C.c_float)]
+                ("vec_alpha", C.c_float), ("vec_distance_threshold", C.c_float), ("vec_flags", C.c_uint32)]
 
     def __init__(self, **kw):
         super().__init__(num_typos=2, prefix=1, max_candidates=4, typo_tokens_threshold=1, drop_tokens_threshold=1, topster_size=250, device_art_walk=1,
-                         n_threads=0, vec_k=0, vec_ef=10, vec_flat_search_cutoff=0, vec_fetch_size=10, vec_alpha=0.3, vec_distance_threshold=3.4028234663852886e38)
+                         n_threads=0, vec_k=0, vec_ef=10, vec_flat_search_cutoff=0, vec_fetch_size=10, vec_alpha=0.3, vec_distance_threshold=3.4028234663852886e38,
+                         vec_flags=0)
         for k, v in kw.items():
             setattr(self, k, v)
 

@@ -80,7 +80,8 @@ class StatsStruct(C.Structure):
                 ("knn_tier2_walks", C.c_uint64), ("knn_retried", C.c_uint64), ("h2d_total", C.c_uint64), ("d2h_total", C.c_uint64),
                 ("calls_total", C.c_uint64), ("knn_table_probes", C.c_uint64), ("flat_tc_queries", C.c_uint64),
                 ("deep_entries", C.c_uint64), ("deep_bytes", C.c_uint64), ("ms_deep_emit", C.c_float), ("ms_deep_dedup", C.c_float),
-                ("ms_deep_select", C.c_float), ("pad_deep", C.c_float)]
+                ("ms_deep_select", C.c_float), ("pad_deep", C.c_float), ("deep_fuse_bytes", C.c_uint64), ("ms_deep_fuse_prep", C.c_float),
+                ("ms_deep_fuse_replay", C.c_float), ("ms_deep_fuse_rerank", C.c_float), ("ms_deep_fuse_sort", C.c_float)]
 
 
 def _ptr(a: Optional[np.ndarray], typ):
@@ -305,6 +306,7 @@ class HnswGraph:
 
 
 VEC_FLAT_TENSOR = 1
+VEC_DEEP_TOPSTER = 2          # q_topk > MAX_TOPK (with FLAG_DEEP_TOPSTER) and hybrid k up to 4096 in the vector / hybrid calls
 
 
 def vec_params(k=0, ef=10, flat_search_cutoff=0, distance_threshold=3.4028234663852886e38, alpha=0.3, fetch_size=10, flags=0):
