@@ -471,7 +471,7 @@ typedef struct {
     float    ms_knn;             /* HNSW / flat kernels */
     float    ms_fuse;            /* RRF / final top-k kernels */
     uint64_t launches_total;     /* kernels launched by this library since index creation */
-    uint64_t kw_driver_ids;      /* candidate (driver-list) ids scanned */
+    uint64_t kw_driver_ids;      /* candidate ids scanned: driver-list ids, or the documents a bitmap tile covers (all-dense combinations) */
     uint64_t kw_probe_ids;       /* posting ids covered by probed blocks */
     uint64_t kw_matches;         /* docs scored */
     uint64_t knn_dist;           /* distance evaluations */

@@ -72,7 +72,7 @@ struct CDesc {
     uint32_t drv_tile_off[kMaxFieldSlots + 1];
     uint8_t  probe_order[16];
     uint32_t mode;                     // 0: driver tiles + per-candidate probes; 1: word-parallel AND of dense bitmaps
-    uint32_t n_words;                  // mode 1: valid bitmap words = ceil(n_docs / 32)
+    uint32_t w_begin, w_end;           // mode 1: bitmap words [w_begin, w_end) the tiles cover; w_begin is a multiple of 32
 };
 
 struct UDesc {
@@ -401,12 +401,14 @@ kw_search_kernel(const __grid_constant__ IndexDev ix, const __grid_constant__ Kw
 
     if(cd.mode == 1) {
         // ---- all required tokens are dense lists: intersect their bitmaps 32 docs per instruction. A tile is 128
-        // consecutive bitmap words (4096 docs), one word per thread; set bits are popped one per thread and round into
-        // the same scoring queue. Replaces the whole decode/narrow/probe pipeline for the heaviest combinations.
+        // consecutive bitmap words (4096 docs) of the lists' common id range, one word per thread; set bits are popped one
+        // per thread and round into the same scoring queue. Replaces the decode/narrow/probe pipeline for the heaviest
+        // combinations.
         for(uint32_t tile = ud.tile_begin; tile < ud.tile_end; tile++) {
-            const uint32_t wi = tile * kThreads + tid;
+            const uint32_t w0 = cd.w_begin + tile * kThreads, wi = w0 + tid;
             uint32_t word = 0;
-            if(wi < cd.n_words && !qd.filter_empty) {
+            if(tid == 0) s_driver_ids += (min(cd.w_end - w0, (uint32_t) kThreads)) << 5;      // documents the tile covers
+            if(wi < cd.w_end && !qd.filter_empty) {
                 word = 0xFFFFFFFFu;
                 for(uint32_t r = 0; r < cd.n_rows; r++) {
                     if(!((cd.req_mask >> r) & 1)) continue;

@@ -113,6 +113,7 @@ struct FieldMirror {
     std::vector<uint64_t> h_list_off;
     std::vector<uint32_t> h_list_blk_off;
     std::vector<uint32_t> h_list_dense;
+    std::vector<uint32_t> h_list_first, h_list_last;   // smallest / largest id of each list (the bitmap path's word range)
     void* d_alloc[10] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     // element counts of the device arrays (tsgpu_index_append_lists grows them)
     size_t d_bytes[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};   // bytes allocated per array (tsgpu_index_field_info)
@@ -184,6 +185,16 @@ constexpr uint32_t kMergeFan = 16;
 
 uint32_t pow2_ceil(uint32_t v) { uint32_t p = 1; while(p < v) p <<= 1; return p; }
 
+// appends the first and last id of lists [0, n) (offsets list_off[] - base into ids[]); an empty list gets first > last
+void list_id_range(uint32_t n, const uint64_t* list_off, const uint32_t* ids, uint64_t base, std::vector<uint32_t>& first,
+                   std::vector<uint32_t>& last) {
+    for(uint32_t l = 0; l < n; l++) {
+        const uint64_t a = list_off[l] - base, b = list_off[l + 1] - base;
+        first.push_back(b > a ? ids[a] : kNone);
+        last.push_back(b > a ? ids[b - 1] : 0);
+    }
+}
+
 // ------------------------------------------------------------------------------------------------- keyword prep
 struct KwPlan {
     uint32_t nq = 0, nc = 0, F = 0, n_units = 0;
@@ -237,6 +248,7 @@ tsgpu_status build_kw_plan(tsgpu_index* idx, const tsgpu_kw_batch* b, bool with_
         return fm.h_list_off[l + 1] - fm.h_list_off[l];
     };
     // ---- combos
+    const double dense_cost = getenv("TSGPU_DENSE_COST") ? atof(getenv("TSGPU_DENSE_COST")) : 0.5;   // read per call: tools/bench_dense_kw.py sweeps it
     std::vector<uint32_t> combo_tiles(pl.nc, 0);
     uint64_t total_tiles = 0;
     for(uint32_t c = 0; c < pl.nc; c++) {
@@ -271,29 +283,33 @@ tsgpu_status build_kw_plan(tsgpu_index* idx, const tsgpu_kw_batch* b, bool with_
         for(uint32_t r = 0; r < n_req; r++) if(sumdf[r]) { cd.req_mask |= 1u << r; if(drv == kNone || sumdf[r] < sumdf[drv]) drv = r; }
         uint32_t tiles = 0;
         for(uint32_t f = 0; f <= (uint32_t) kMaxFieldSlots; f++) cd.drv_tile_off[f] = 0;
-        cd.mode = 0; cd.n_words = (uint32_t) (((uint64_t) idx->n_docs + 31) / 32);
-        static const bool dense_mode_on = getenv("TSGPU_DENSE_MODE") && atoi(getenv("TSGPU_DENSE_MODE")) == 1;   // opt-in: measured slower at 10 M docs
-        bool all_dense = drv != kNone && dense_mode_on;
+        cd.mode = 0; cd.w_begin = cd.w_end = 0;
+        // Every required token dense: the bitmap AND reads each word of the id range once per list, the driver tiles probe
+        // every driver id. Take the bitmaps when the words are fewer than dense_cost x the driver ids (DESIGN.md §3).
+        bool all_dense = drv != kNone;
+        uint32_t id_lo = 0, id_hi = idx->n_docs ? idx->n_docs - 1 : 0;     // docs every required row can hold
         for(uint32_t r = 0; r < n_req && all_dense; r++) {
             if(!((cd.req_mask >> r) & 1)) continue;
+            uint32_t row_lo = kNone, row_hi = 0;
             for(uint32_t f = 0; f < F; f++) {
                 const uint32_t l = cd.lists[r * F + f];
-                if(l != TSGPU_NO_LIST && idx->fields[b->field_ids[f]].h_list_dense[l] == kNone) { all_dense = false; break; }
+                if(l == TSGPU_NO_LIST) continue;
+                const FieldMirror& fm = idx->fields[b->field_ids[f]];
+                if(fm.h_list_dense[l] == kNone) { all_dense = false; break; }
+                row_lo = std::min(row_lo, fm.h_list_first[l]); row_hi = std::max(row_hi, fm.h_list_last[l]);
             }
+            id_lo = std::max(id_lo, row_lo); id_hi = std::min(id_hi, row_hi);
         }
-        // candidate-mode tiles of the driver vs word tiles of the whole id space: a word tile is ~3x cheaper than a
-        // candidate tile, so the bitmap AND only pays when the driver itself covers a good part of the collection
-        uint32_t cand_tiles = 0;
-        if(drv != kNone) for(uint32_t f = 0; f < F; f++) {
-            const uint32_t l = cd.lists[drv * F + f];
-            if(l != TSGPU_NO_LIST) cand_tiles += (uint32_t) ((df_of(f, l) + tsdev::kBlock - 1) / tsdev::kBlock);
-        }
-        if(all_dense && cand_tiles < 2 * ((cd.n_words + kThreads - 1) / kThreads)) all_dense = false;
         if(all_dense) {
-            // every required token is a dense list: word-parallel bitmap AND over the whole id space (kw_kernels.cuh)
+            cd.w_begin = (id_lo >> 5) & ~31u;                          // 128-byte aligned loads
+            cd.w_end = id_lo <= id_hi ? (id_hi >> 5) + 1 : cd.w_begin;
+            if((double) (cd.w_end - cd.w_begin) >= dense_cost * (double) sumdf[drv]) all_dense = false;
+        }
+        if(all_dense) {
+            // word-parallel bitmap AND over [w_begin, w_end) (kw_kernels.cuh)
             cd.mode = 1;
             cd.driver_row = (uint8_t) drv;
-            tiles = (cd.n_words + kThreads - 1) / kThreads;
+            tiles = (cd.w_end - cd.w_begin + kThreads - 1) / kThreads;
             for(uint32_t f = 0; f <= (uint32_t) kMaxFieldSlots; f++) cd.drv_tile_off[f] = f == 0 ? 0 : tiles;
             for(uint32_t i = 0; i < 16; i++) cd.probe_order[i] = (uint8_t) (i < n_rows ? i : 0);
         } else if(drv != kNone) {
@@ -1315,6 +1331,8 @@ tsgpu_status tsgpu_index_load_field(tsgpu_index* idx, const tsgpu_field* f, uint
     // dense lists: bitmap + rank directory (see postings_device.cuh)
     tspack::pack_dense(L, fm.h_list_off.data(), h_ids.data(), idx->n_docs, fm.dense_min_df, pk);
     fm.h_list_dense = pk.list_dense;
+    fm.h_list_first.clear(); fm.h_list_last.clear();
+    list_id_range(L, fm.h_list_off.data(), h_ids.data(), 0, fm.h_list_first, fm.h_list_last);
     CU(up(7, pk.list_dense.data(), pk.list_dense.size() * 4, false));
     CU(up(8, pk.dense_bits.data(), pk.dense_bits.size() * 4, false));
     CU(up(9, pk.dense_rank.data(), pk.dense_rank.size() * 4, false));
@@ -1437,6 +1455,7 @@ tsgpu_status tsgpu_index_append_lists(tsgpu_index* idx, uint32_t field, const ts
     fm.h_list_blk_off.insert(fm.h_list_blk_off.end(), pk.list_blk_off.begin() + 1, pk.list_blk_off.end());
     fm.h_list_dense.resize(L0);               // (the loader keeps one spare entry for an empty field)
     fm.h_list_dense.insert(fm.h_list_dense.end(), pk.list_dense.begin(), pk.list_dense.begin() + Ln);
+    list_id_range(Ln, lo.data(), ids.data(), fm.n_post, fm.h_list_first, fm.h_list_last);   // lo is rebased by n_post
     fm.n_post += np; fm.n_pos += npos; fm.n_words += nw_new; fm.n_blocks += nb_new; fm.n_dense += pk.n_dense;
     fm.dev.n_lists = L0 + Ln;
     fm.dev.is_array = flags;
